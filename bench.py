@@ -61,7 +61,7 @@ def measured_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1400.0))), 'measured'
-    return 6650.0, 1400.0, 'fallback'
+    return 3350.0, 989.0, 'fallback'     # H100 SXM data sheet: HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
 
 
 class ClockSampler:
@@ -119,7 +119,7 @@ def workload_config(wl_name, wl, batch, world, scaling, graph=True):
             'name': wl_name, 'query_channels': 5 + wl['c_extra'], 'observations': wl['k_obs'],
             'kernel': wl['kernel'], 'depth': wl['depth'], 'global_batch': batch * world, 'uv': uv,
             'parallelism': 'dp%d' % world, 'scaling': scaling, 'cuda_graph': graph,
-            'l2_flush': 'inputs+activations per step (GBs) exceed the 126 MB L2; fresh batch buffers rotate'}
+            'l2_flush': 'inputs+activations per step (GBs) exceed the 50 MB L2; fresh batch buffers rotate'}
 
 
 # ----------------------------------------------------------------------------
@@ -248,7 +248,8 @@ class TrainRun:
         import trainvali
         if self.graphed is not None and not eager:
             return self.graphed(batch)
-        return trainvali.distributed_train_step(self.strategy, self.model, batch, self.opt, self.global_bs)
+        self.last = trainvali.distributed_train_step(self.strategy, self.model, batch, self.opt, self.global_bs)
+        return self.last
 
     def measure_resident(self, steps, warmup):
         import nlt_native as nat
@@ -311,6 +312,29 @@ class TrainRun:
         summ = engine.PROF.summary()
         engine.PROF.enabled = False
         return summ
+
+
+DUMP_SAMPLE = 1 << 21          # elements kept of an output larger than this (fixed seeded sample)
+
+
+def dump_outputs(out_dir, run):
+    """What the timed path computed in its last step, as float32 .npy files: the step's loss, the UV-space network
+    output and the camera-space prediction it returns, and the parameters and their gradients after the step.
+    An output larger than DUMP_SAMPLE elements is reduced to a sample of its elements drawn with a fixed seed (the same
+    indices on every run of the same shape), which keeps the files under 40 MB in all."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    g = run.graphed
+    loss, to_vis = (g.loss, g.to_vis) if g is not None and g.graph is not None else run.last
+    model = run.model
+    arrays = {'loss': loss, 'pred': to_vis['pred'], 'pred_camspc': to_vis['pred_camspc'],
+              'params': model.flat_params, 'grads': model.flat_grads}
+    for name, t in arrays.items():
+        a = t.detach().float().reshape(-1).cpu()
+        if a.numel() > DUMP_SAMPLE:
+            idx = torch.randperm(a.numel(), generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE].sort().values
+            a = a[idx]
+        np.save(os.path.join(out_dir, name + '.npy'), a.numpy())
 
 
 def parity_check(run):
@@ -428,7 +452,7 @@ def sub_record(args):
         ms_e2e, h2d = run.measure_e2e(args.steps)
         rec.update({'ms_per_step': ms, 'value': run.texels / (ms * 1e-3), 'e2e_ms_per_step': ms_e2e,
                     'e2e_value': run.texels / (ms_e2e * 1e-3), 'h2d_bytes_per_step': h2d,
-                    'gpu_launches_per_step': launches / args.steps, 'tcgen05_launches_per_step': tc / args.steps,
+                    'gpu_launches_per_step': launches / args.steps, 'tc_launches_per_step': tc / args.steps,
                     'hbm_frac': wl['bytes'][1] * run.texels / (ms * 1e-3) / 1e9 / peak_gbs,
                     'alg_bytes_per_texel': wl['bytes'][1],
                     'peak_mem_GB': torch.cuda.max_memory_allocated() / 1e9})
@@ -443,7 +467,7 @@ def collect_extra(args):
         name = sub.split(':')[0]
         if name == args.workload and sub.endswith(':%d' % (args.batch or WORKLOADS[name]['batch'])):
             continue
-        cmd = [sys.executable, os.path.abspath(__file__), '--sub', sub, '--steps', str(min(args.steps, 5)),
+        cmd = [sys.executable, os.path.abspath(__file__), '--sub', sub, '--steps', str(args.steps),
                '--warmup', '3']
         try:
             r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.PIPE, timeout=args.sub_timeout)
@@ -472,6 +496,8 @@ def run_b200(args):
     global_bs = batch * world
 
     if not wl['train']:
+        if args.dump_outputs:
+            raise SystemExit('bench.py: --dump-outputs covers the training workloads')
         rec = forward_record(strategy, wl, batch, args.steps, args.warmup)
         if rank == 0:
             emit({'metric': 'UV texels/sec fwd', 'value': rec['value'], 'unit': UNIT, 'n_gpus': world,
@@ -493,6 +519,8 @@ def run_b200(args):
         sampler.start()
     ms_step, launches, tc_launches = run.measure_resident(args.steps, 0)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, run)
 
     # ---- end-to-end arm ----
     ms_e2e, h2d_bytes = run.measure_e2e(args.steps)
@@ -512,8 +540,8 @@ def run_b200(args):
         step_flops = 3.0 * wl['flop_fwd'] * texels_rank
         roof = {
             'bound': 'hbm', 'achieved': ach, 'peak': peak_gbs, 'unit': 'GB/s', 'frac': ach / peak_gbs,
-            'traffic': ncu_traffic(top_label), 'peak_source': how + ' copy bandwidth (MEASURED_PEAKS.json hbm_gbs)'
-            if how == 'measured' else 'fallback 6.65 TB/s (B200_PROFILING.md)',
+            'peak_source': how + ' copy bandwidth (MEASURED_PEAKS.json hbm_gbs)'
+            if how == 'measured' else 'H100 SXM data sheet, 3.35 TB/s',
             'kernel': top_label, 'kernel_launches_per_step': top['launches'] / 2,
             'kernel_ms_per_launch': top['ms'] / top['launches'],
             'kernel_alg_bytes_per_launch': top['bytes'] / top['launches'],
@@ -525,7 +553,7 @@ def run_b200(args):
                      'alg_flops': step_flops,
                      'tf32_peak_tflops_measured': tf32_peak,
                      'flop_frac_of_tf32_peak': step_flops / (ms_step * 1e-3) / 1e12 / tf32_peak,
-                     'flop_note': 'algorithmic conv FLOPs (fwd+bwd = 3 x fwd); the tcgen05 kernels spend 3 TF32 '
+                     'flop_note': 'algorithmic conv FLOPs (fwd+bwd = 3 x fwd); the wgmma kernels spend 3 TF32 '
                                   'products per algorithmic product (3xTF32 split), the fp32 kernels none'},
             'per_op_sum_ms': total_ms / 2,
             'top5': sorted(((k, round(v['ms'] / 2, 4)) for k, v in summ.items()), key=lambda kv: -kv[1])[:5],
@@ -586,7 +614,7 @@ def run_b200(args):
                                      'note': 'same call with the image tensors as uint8 PNG samples (datasets '
                                              'uint8_inputs = True; v / 255 on the device, bit-identical results); the '
                                              'float32 number above is bounded by PCIe (h2d bytes / step time)'}},
-            'gpu_launches': launches, 'tcgen05_launches': tc_launches,
+            'gpu_launches': launches, 'tc_launches': tc_launches,
             'whole_step_in_cuda_graph': bool(run_graph_full), 'clocks': clocks, 'parity': parity,
             'roofline': roof, 'cpu_baseline': cpu,
         }
@@ -597,17 +625,6 @@ def run_b200(args):
         emit(line)
     if world > 1:
         torch.distributed.destroy_process_group()
-
-
-def ncu_traffic(label):
-    """DRAM bytes per launch of the dominant kernel, from the committed ncu --set full capture
-    (profiles/ncu_traffic.json); None when that kernel has not been captured."""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'ncu_traffic.json')) as f:
-            ent = json.load(f).get(label)
-        return float(ent['dram_bytes_per_launch']) if ent else None
-    except (OSError, ValueError, KeyError):
-        return None
 
 
 _JSON_OUT = None
@@ -646,6 +663,8 @@ def main():
     ap.add_argument('--no-parity', action='store_true', help='skip the in-bench parity gate')
     ap.add_argument('--no-graph', dest='no_graph', action='store_true', help='launch kernels eagerly (no CUDA graph)')
     ap.add_argument('--profile-out', dest='profile_out', default=None, help='write the per-op device-time table here')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step to DIR/<name>.npy (float32)')
     ap.add_argument('--sub', default=None, help=argparse.SUPPRESS)
     ap.add_argument('--sub-timeout', dest='sub_timeout', type=int, default=240, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -654,7 +673,7 @@ def main():
         run_reference(args)
         return
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py: no CUDA device (the B200 path has no CPU fallback); '
+        raise SystemExit('bench.py: no CUDA device (the CUDA path has no CPU fallback); '
                          'use --impl reference for the CPU arm')
     if args.sub:
         sub_record(args)

@@ -1,9 +1,9 @@
-/* nlt_b200.h -- C ABI of the B200-native NLT UV-space hot path.
+/* nlt_b200.h -- C ABI of the NLT UV-space hot path (sm_90a).
  *
  * The reference (google/neural-light-transport) has NO native/FFI boundary:
  * its numerics live in pip wheels (tensorflow 2.2 / tensorflow-addons 0.10)
  * called from Keras layers.  Each entry point below therefore cites the
- * reference *call site* it replaces (paths relative to /root/reference).
+ * reference *call site* it replaces (paths relative to the reference checkout).
  *
  * Conventions
  *  - every pointer is a DEVICE pointer to fp32, NHWC contiguous, owned by the
@@ -69,7 +69,8 @@ typedef struct nlt_gconv_desc {
 } nlt_gconv_desc;
 
 const char* nlt_version(void);
-/* process-wide switches: "tc" (1: tcgen05 3xTF32 path where eligible [default], 0: fp32-FMA kernels only),
+/* process-wide switches: "tc" (1: wgmma 3xTF32 path where eligible [default], 0: fp32-FMA kernels only, 2: the wgmma
+ * path for every shape it can run, ahead of the size heuristics and the stream kernels -- for A/B tests),
  * "tc_wgrad" (same for the weight-gradient kernel), "wgrad_rows" (1: row-run form of the warp-stream
  * weight-gradient kernel where float4 access allows it [default], 0: flat-pixel form), "dconv_wide" (1: the
  * pixel x 16-outputs stencil kernel for the 16-channel stencils, 0: the tiled implicit-GEMM kernel),
@@ -82,7 +83,10 @@ int nlt_set_option(const char* name, int value);
 const char* nlt_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process (diagnostic counter) */
 uint64_t nlt_launch_count(void);
-/* how many of those were tcgen05 tensor-core kernels (diagnostic counter) */
+/* launches of one kernel so far, by the name the library reports it under (e.g. "pf_fwd_kernel"); 0 if never
+ * launched (diagnostic counter: lets tests check which kernel a routing option selected) */
+uint64_t nlt_kernel_launch_count(const char* name);
+/* how many of those were wgmma tensor-core kernels (diagnostic counter) */
 uint64_t nlt_tc_launch_count(void);
 
 /* out = act(A*W + bias);   then  out = beta*out_old + out;  then out *= act'(mask_y)
@@ -92,9 +96,9 @@ uint64_t nlt_tc_launch_count(void);
 int nlt_gconv_fwd(const nlt_gconv_desc* d, const float* bias, int act,
                   float beta, const float* mask_y, int mask_act,
                   float* out, void* stream);
-/* Same op with caller-provided scratch: enables the tcgen05 (3xTF32 split,
- * fp32 accumulate in TMEM) tensor-core path where the shape allows it (all
- * sources with C % 32 == 0, Cout % 16 == 0, tileable lattice); the scratch holds
+/* Same op with caller-provided scratch: enables the wgmma (3xTF32 split,
+ * fp32 accumulate in registers) tensor-core path where the shape allows it (all
+ * sources with C % 16 == 0, Cout % 16 == 0, tileable lattice); the scratch holds
  * the per-call hi/lo TF32 weight planes.  Falls back to the fp32 kernels
  * otherwise.  Set NLT_DISABLE_TC=1 in the environment to force the fp32 path. */
 int64_t nlt_gconv_fwd_workspace_bytes(const nlt_gconv_desc* d);
@@ -233,11 +237,6 @@ int nlt_instnorm_fwd(const float* x, const float* gamma, const float* beta, int3
 int nlt_instnorm_bwd(const float* x, const float* dz, const float* gamma, const float* mean, const float* rstd,
                      int32_t N, int32_t HW, int32_t C, float* dx, float* dgamma, float* dbeta, int accumulate,
                      void* workspace, void* stream);
-
-/* Diagnostic (tests/test_gpu_tcts.py): out[128 x bn] = A[128 x 16] * B[bn x 16]^T through the TS form of
- * tcgen05.mma (A operand written to tensor memory with tcgen05.st, B in shared memory); bn = 16 or 32.
- * A is fed unrounded, so the result shows how the tensor core treats the low 13 mantissa bits of fp32 inputs. */
-int nlt_debug_tcts_probe(const float* A, const float* B, int32_t bn, float* out, void* stream);
 
 /* uint8 image samples -> float32 in [0, 1] (v / 255, correctly rounded = the host pipeline's
  * float32(v / 255.0), nlt/datasets/nlt.py:134-139): lets a batch cross PCIe as bytes (SURVEY 8f N3). */

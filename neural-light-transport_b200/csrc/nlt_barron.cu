@@ -1,6 +1,6 @@
 // "barron" training-loss term of NLT (nlt/losses.py:90-121) fused with its gradient -- SURVEY.md 8f, row N1.
-// EXPERIMENTAL: written after round 1's GPU budget was spent; the per-element arithmetic (nlt_barron_core.h) is
-// checked on the CPU against the pinned oracle, the kernels themselves have not run on hardware yet.
+// The per-element arithmetic (nlt_barron_core.h) is checked on the CPU against the pinned oracle, the kernels by
+// tests/test_gpu_barron.py.
 //
 // Planar fp32 scratch ([3B planes][rows][cols]); per level l (image A x B):
 //   rows pass : L[ceil(A/2)][B], H[floor(A/2)][B]

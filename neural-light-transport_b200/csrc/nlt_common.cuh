@@ -1,4 +1,4 @@
-// Shared device/host helpers for the NLT B200 kernels.
+// Shared device/host helpers for the NLT kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,9 +14,19 @@ int set_err(int code, const char* fmt, ...);
 #define NLT_CHECK_ARG(cond, ...) \
   do { if (!(cond)) return nlt::set_err(NLT_ERR_INVALID, __VA_ARGS__); } while (0)
 extern unsigned long long g_launches;   // kernels launched by this library (diagnostic only)
+void count_launch(const char* what);    // per-kernel launch counter behind nlt_kernel_launch_count (diagnostic only)
 #define NLT_CUDA_LAUNCH_CHECK(what) \
-  do { __atomic_add_fetch(&nlt::g_launches, 1ull, __ATOMIC_RELAXED); cudaError_t e_ = cudaGetLastError(); \
+  do { __atomic_add_fetch(&nlt::g_launches, 1ull, __ATOMIC_RELAXED); nlt::count_launch(what); \
+       cudaError_t e_ = cudaGetLastError(); \
        if (e_ != cudaSuccess) return nlt::set_err(NLT_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e_)); } while (0)
+
+// SMs of the current device: grid caps of the grid-stride and persistent kernels (cached per device)
+int sm_count();
+
+// two fp32 FMAs on a float pair (a * b + c per component, round-to-nearest)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
+}
 
 // ---- division by an invariant (Granlund-Montgomery), n < 2^31 ----------------
 struct FastDiv {
@@ -38,7 +48,7 @@ __device__ __forceinline__ uint32_t fdiv(uint32_t n, const FastDiv& f) {
 // ---- activation ---------------------------------------------------------------
 // forward (nlt/networks/elements.py:69-78).  `act` is warp-uniform: the piecewise-linear cases cost
 // three instructions per value; ELU (expm1f) sits behind a real call so that its ~30 instructions are
-// not if-converted into every epilogue (they were: ncu showed the epilogues dominating the small kernels).
+// not if-converted into every epilogue.
 static __device__ __noinline__ float elu_slow(float x) { return x > 0.f ? x : expm1f(x); }
 __device__ __forceinline__ float act_fwd(float x, int act) {
   if (act == NLT_ACT_ELU) return elu_slow(x);
@@ -143,7 +153,7 @@ int launch_pw_conv(const GConvK& k, const float* bias, int act, float beta, cons
 // wide stencil kernel (pixel x 16 outputs per thread); option "dconv_wide" / NLT_DCONV_WIDE
 #define NLT_DCONV_WIDE_DEFAULT 1
 extern int g_opt_dconv_wide;
-extern int g_opt_dconv_cw;       // constant-memory weight table + FFMA2 form of the wide stencil kernel: 1 on (default)
+extern int g_opt_dconv_cw;       // constant-memory weight table form of the wide stencil kernel: 1 on (default)
 extern int g_opt_dconv_wide8;    // experimental 8-output form: 0 off (default), 1 on
 extern int g_opt_dconv_wide32;   // experimental 32-output form: 0 off (default), 1 one pixel / thread, 2 two pixels
 bool dconv_wide_applicable(const GConvK& k, const float* out, const float* mask_y);
@@ -196,14 +206,15 @@ bool pwd2s_applicable(const GConvK& k, const float* bias, int act, const float* 
 int launch_pwd2s(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
                  const PwExtra* ex);
 
-// weight gradient of the 2x2 convs of the 16- / 32-channel levels (staged input patch + FFMA2, nlt_pwx.cu)
+// weight gradient of the 2x2 convs of the 16- / 32-channel levels (staged input patch, nlt_pwx.cu)
 bool pws_wgrad_applicable(const GConvK& k, const float* G);
 size_t pws_wgrad_ws_floats(const GConvK& k);
 int launch_pws_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size_t* KD_pad, cudaStream_t st);
 
-// tcgen05 tensor-core path (nlt_tc.cu)
-#define NLT_TCS_DEFAULT 0
-extern int g_opt_tcs;            // TS form of the forward kernel (A operand through tensor memory)
+// wgmma tensor-core path (nlt_tc.cu)
+#define NLT_TCS_DEFAULT 1
+extern int g_opt_tcs;            // register form of the forward kernel (A operand split in registers, wgmma RS)
+extern int g_tc_force;           // option "tc" = 2: the tensor-core kernel for every shape it can run (A/B testing)
 extern unsigned long long g_tc_launches;
 bool tc_applicable(const GConvK& k);
 size_t tc_workspace_bytes(const GConvK& k);

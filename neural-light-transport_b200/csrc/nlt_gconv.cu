@@ -8,10 +8,11 @@
 // activation-derivative mask are fused into the epilogue.
 //
 // Bound: for Cout <= 16 these layers are HBM-bound (AI ~ 4-7 FLOP/B); for
-// larger Cout this fp32-FFMA path is FMA-bound and the tcgen05 path
+// larger Cout this fp32-FFMA path is FMA-bound and the wgmma path
 // (nlt_tc.cu) takes over where the shape allows.
 #include <stdlib.h>
 #include <string.h>
+#include <mutex>
 #include "nlt_common.cuh"
 
 namespace nlt {
@@ -27,6 +28,18 @@ int set_err(int code, const char* fmt, ...) {
   return code;
 }
 
+int sm_count() {
+  static int n[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (n[dev] == 0) {
+    int v = 0;
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    n[dev] = v > 0 ? v : 132;
+  }
+  return n[dev];
+}
 
 int build_phases(const nlt_gconv_desc* d, GConvK* out, int* nphase, bool allow_d2s) {
   NLT_CHECK_ARG(d != nullptr, "null descriptor");
@@ -572,9 +585,9 @@ gconv_wgrad_reduce_kernel(const WgradK w, const float* __restrict__ ws, size_t K
   }
 }
 
-// Few partials (the tcgen05 wgrad of the deep levels: 2-32 splits of a [K_d x N] matrix of up to 4096 x 256):
+// Few partials (the wgmma wgrad of the deep levels: 2-32 splits of a [K_d x N] matrix of up to 4096 x 256):
 // one thread per output, splits summed serially in fixed order.  The 32-lane form above keeps 2 of its 32 split
-// lanes busy there and took 45-160 us per launch (ncu launch list, profiles/r1_l) for 2 MB of partials.
+// lanes busy there, tens of microseconds per launch for 2 MB of partials.
 __global__ void __launch_bounds__(256)
 gconv_wgrad_reduce_flat_kernel(const WgradK w, const float* __restrict__ ws, size_t KD_pad,
                                float* __restrict__ dW, float* __restrict__ db, int acc_w, int acc_b) {
@@ -630,9 +643,9 @@ static WgradPlan plan_wgrad(const GConvK& k) {
   p.n_tiles = (k.Cout + p.tn - 1) / p.tn;
   p.ld = (k.Cout + 3) / 4 * 4;
   p.KD_pad = (size_t)p.kd_tiles * p.tkg * 4;
-  // enough CTAs to fill 148 SMs a few times over, at least 64 pixels per CTA
+  // enough CTAs to fill every SM a few times over, at least 64 pixels per CTA
   const long long tiles = (long long)p.kd_tiles * p.n_tiles;
-  long long want = (148ll * 8 + tiles - 1) / tiles;
+  long long want = ((long long)sm_count() * 8 + tiles - 1) / tiles;
   long long max_split = ((long long)k.M + 63) / 64;
   if (want > max_split) want = max_split;
   if (want < 1) want = 1;
@@ -650,24 +663,49 @@ static WgradPlan plan_wgrad(const GConvK& k) {
 
 using namespace nlt;
 
+namespace nlt {
+// launches per kernel label (the string literal of NLT_CUDA_LAUNCH_CHECK; about 60 labels in the library)
+static std::mutex g_kl_mutex;
+static const char* g_kl_name[128];
+static uint64_t g_kl_count[128];
+static int g_kl_n = 0;
+void count_launch(const char* what) {
+  std::lock_guard<std::mutex> lock(g_kl_mutex);
+  for (int i = 0; i < g_kl_n; ++i)
+    if (g_kl_name[i] == what || strcmp(g_kl_name[i], what) == 0) { ++g_kl_count[i]; return; }
+  if (g_kl_n < 128) { g_kl_name[g_kl_n] = what; g_kl_count[g_kl_n++] = 1; }
+}
+}  // namespace nlt
+
 extern "C" {
 
-const char* nlt_version(void) { return "nlt_b200 0.1 (sm_100a)"; }
+const char* nlt_version(void) { return "nlt_b200 0.1 (sm_90a)"; }
 const char* nlt_last_error(void) { return nlt::g_err; }
 uint64_t nlt_launch_count(void) { return __atomic_load_n(&nlt::g_launches, __ATOMIC_RELAXED); }
+
+uint64_t nlt_kernel_launch_count(const char* name) {
+  if (name == nullptr) return 0;
+  std::lock_guard<std::mutex> lock(nlt::g_kl_mutex);
+  for (int i = 0; i < nlt::g_kl_n; ++i)
+    if (strcmp(nlt::g_kl_name[i], name) == 0) return nlt::g_kl_count[i];
+  return 0;
+}
 uint64_t nlt_tc_launch_count(void) { return __atomic_load_n(&nlt::g_tc_launches, __ATOMIC_RELAXED); }
 
 static int g_opt_tc = -1, g_opt_tc_wgrad = -1;   // -1: take the environment default
-// option "pwd2s_first" / NLT_PWD2S_FIRST (default 1): level-3 input gradients 0.364 -> 0.341 and 0.185 -> 0.170 ms
-// (profiles/r2_y_*)
+// option "pwd2s_first" / NLT_PWD2S_FIRST (default 0): the pointwise depth-to-space kernel ahead of the wgmma kernel for
+// the input gradients of 2x2/s2 convs from 64-channel sources.  H100, cfg4 step: the wgmma kernel is faster there
+// (level-3 input gradients 0.64 ms less per step)
 static int g_opt_pwd2s_first = -1;
 static bool pwd2s_first() {
-  if (g_opt_pwd2s_first < 0) { const char* e = getenv("NLT_PWD2S_FIRST"); g_opt_pwd2s_first = (e && e[0] == '0') ? 0 : 1; }
+  if (g_opt_pwd2s_first < 0) { const char* e = getenv("NLT_PWD2S_FIRST"); g_opt_pwd2s_first = (e && e[0] == '1') ? 1 : 0; }
   return g_opt_pwd2s_first == 1;
 }
-static int g_opt_pf = -1;                        // option "pf" / NLT_PF (default 1): staged-patch forward of nlt_pwx.cu
+// option "pf" / NLT_PF (default 0): staged-patch forward of nlt_pwx.cu.  H100, cfg4 step: the level-1/2 forward convs
+// take 0.87 ms less on the general kernels
+static int g_opt_pf = -1;
 static bool pf_enabled() {
-  if (g_opt_pf < 0) { const char* e = getenv("NLT_PF"); g_opt_pf = (e && e[0] == '0') ? 0 : 1; }
+  if (g_opt_pf < 0) { const char* e = getenv("NLT_PF"); g_opt_pf = (e && e[0] == '1') ? 1 : 0; }
   return g_opt_pf == 1;
 }
 static int g_opt_dconv_wide_first = -1;          // routing switch (NLT_DCONV_WIDE_FIRST, default 1), see nlt_gconv_fwd_ws
@@ -680,9 +718,8 @@ static bool tc_enabled() {
   return g_opt_tc == 1;
 }
 
-// tensor-core weight gradient for this phase?  Measured (profiles/r1_j): the row-run warp-stream kernel
-// beats the tcgen05 one when it applies at all (<= 16 gradient channels, K-depth <= 160: the level-1
-// 32 -> 16 down-conv, 0.70 vs 0.84 ms), the tcgen05 kernel wins everywhere else.
+// tensor-core weight gradient for this phase?  The row-run warp-stream kernel takes the shapes it applies to
+// (<= 16 gradient channels, K-depth <= 160: the level-1 32 -> 16 down-conv), the wgmma kernel everything else.
 static bool tc_wgrad_enabled();
 static bool use_tc_wgrad(const GConvK& k) {
   return tc_wgrad_enabled() && tc_wgrad_applicable(k) && !wgrad_small_applicable(k);
@@ -695,7 +732,7 @@ static bool tc_wgrad_enabled() {
 
 int nlt_set_option(const char* name, int value) {
   NLT_CHECK_ARG(name != nullptr, "null option name");
-  if (strcmp(name, "tc") == 0) { g_opt_tc = value ? 1 : 0; return NLT_OK; }
+  if (strcmp(name, "tc") == 0) { g_opt_tc = value ? 1 : 0; nlt::g_tc_force = value == 2; return NLT_OK; }
   if (strcmp(name, "tc_wgrad") == 0) { g_opt_tc_wgrad = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "wgrad_rows") == 0) { nlt::g_opt_wgrad_rows = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "tcs") == 0) { nlt::g_opt_tcs = value ? 1 : 0; return NLT_OK; }
@@ -724,10 +761,11 @@ int64_t nlt_gconv_fwd_workspace_bytes(const nlt_gconv_desc* d) {
   return 0;
 }
 
-// does the forward of `d` run on the tcgen05 kernel (which reads packed hi / lo weight planes)?  Mirrors the routing
+// does the forward of `d` run on the wgmma kernel (which reads packed hi / lo weight planes)?  Mirrors the routing
 // order of gconv_fwd_impl below.
 static bool fwd_takes_tc(const GConvK* ph, int np, float beta, const float* mask_y, const float* out) {
   if (np != 1 || ph[0].M == 0) return false;
+  if (g_tc_force) return tc_enabled() && tc_applicable(ph[0]);
   if (pf_enabled() && pf_fwd_applicable(ph[0], mask_y, out)) return false;
   if (tiny_stencil_applicable(ph[0], out, mask_y)) return false;
   if (pwx_d2s_fwd_applicable(ph[0], beta, mask_y, out)) return false;
@@ -777,18 +815,21 @@ static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, f
   NLT_CHECK_ARG(act >= 0 && act <= 3 && mask_act >= 0 && mask_act <= 3, "bad activation code");
   NLT_CHECK_ARG(beta == 0.f || beta == 1.f, "beta must be 0 or 1");
   cudaStream_t st = (cudaStream_t)stream;
+  if (np == 1 && g_tc_force && workspace != nullptr && tc_enabled() && ph[0].M > 0 && tc_applicable(ph[0]) &&
+      (int64_t)tc_workspace_bytes(ph[0]) <= workspace_bytes)
+    return launch_tc(ph[0], bias, act, beta, mask_y, mask_act, out, workspace, (size_t)workspace_bytes, st, prepacked);
   // few-channel stride-1 stencils (4/8/16 -> same): the row-stream kernel of nlt_tiny.cu, ahead of the tensor path
-  // (16 -> 16 at 512^2 is a 130 B/pixel stream: the tcgen05 pipeline's fixed costs exceed its 0.5 kFMA/pixel)
+  // (16 -> 16 at 512^2 is a 130 B/pixel stream: the wgmma pipeline's fixed costs exceed its 0.5 kFMA/pixel)
   if (np == 1 && ph[0].M > 0 && pf_enabled() && pf_s1_level() > 0 && ph[0].ay.it == 1 && pf_fwd_applicable(ph[0], mask_y, out))
     return launch_pf_fwd(ph[0], bias, act, beta, mask_y, mask_act, out, st);
   if (np == 1 && ph[0].M > 0 && tiny_stencil_applicable(ph[0], out, mask_y))
     return launch_tiny_stencil(ph[0], bias, act, beta, mask_y, mask_act, out, st);
-  // 2x2 / stride-2 convs of levels 1-2 (K = 64 / 128 into 16 / 32 channels): staged-patch FFMA2 forward (nlt_pwx.cu)
+  // 2x2 / stride-2 convs of levels 1-2 (K = 64 / 128 into 16 / 32 channels): staged-patch forward (nlt_pwx.cu, option "pf")
   if (np == 1 && pf_enabled() && pf_fwd_applicable(ph[0], mask_y, out))
     return launch_pf_fwd(ph[0], bias, act, beta, mask_y, mask_act, out, st);
   // up-convs into 4 / 8 channels: depth-to-space pointwise kernel with constant-bank weights (nlt_pwx.cu)
   if (np == 1 && pwx_d2s_fwd_applicable(ph[0], beta, mask_y, out)) return launch_pwx_d2s_fwd(ph[0], bias, act, out, st);
-  // input gradients of the 2x2 / stride-2 convs into 32-channel sources with K = 64 (level 3): depth-to-space FFMA2
+  // input gradients of the 2x2 / stride-2 convs into 32-channel sources with K = 64 (level 3): depth-to-space
   // kernel ahead of the tensor path (option "pwd2s_first" / NLT_PWD2S_FIRST)
   if (!prepacked && np == 1 && ph[0].M > 0 && pwd2s_first() && ph[0].d2s && ph[0].nseg == 1 && ph[0].seg[0].C == 64 &&
       pwd2s_applicable(ph[0], bias, act, out, mask_y, nullptr))
@@ -807,8 +848,7 @@ static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, f
     else if (pwd2s_applicable(k, bias, act, out, mask_y, nullptr)) rc = launch_pwd2s(k, beta, mask_y, mask_act, out, st, nullptr);
     else if (pw_conv_applicable(k)) rc = launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, st);
     else if (tiny_stencil_applicable(k, out, mask_y)) rc = launch_tiny_stencil(k, bias, act, beta, mask_y, mask_act, out, st);
-    // option "dconv_wide_first" (default on; measured -0.4 ms per cfg2 step together with the 8-output form,
-    // profiles/r2_a_*): prefer the wide stencil kernel over the quad-per-thread one where both apply
+    // option "dconv_wide_first" (default on): prefer the wide stencil kernel over the quad-per-thread one where both apply
     // (16 / 8 outputs, K <= 32: the up-conv input gradients of levels 11-12)
     else if (dconv_wide_first() && dconv_small_applicable(k) && dconv_wide_applicable(k, out, mask_y))
       rc = launch_dconv_wide(k, bias, act, beta, mask_y, mask_act, out, st);
@@ -895,7 +935,7 @@ int nlt_gconv_wgrad(const nlt_gconv_desc* d, const float* G, float* dW, float* d
   int rc = build_phases(d, ph, &np, /*allow_d2s=*/true);
   if (rc != NLT_OK) return rc;
   // a k == stride transposed conv keeps its one-pass depth-to-space form when a kernel takes it (the warp-stream
-  // kernel for narrow tiles, the tcgen05 kernel from K_d = 128 up); otherwise s*s phases
+  // kernel for narrow tiles, the wgmma kernel from K_d = 128 up); otherwise s*s phases
   if (np == 1 && ph[0].d2s && !pwx_wgrad_applicable(ph[0], G) && !wop_wgrad_applicable(ph[0], G) &&
       !wgrad_small_applicable(ph[0]) && !use_tc_wgrad(ph[0]))
     rc = build_phases(d, ph, &np, false);
@@ -959,7 +999,7 @@ int nlt_gconv_wgrad(const nlt_gconv_desc* d, const float* G, float* dW, float* d
                                                                                      bias_done ? 1 : accumulate);
     } else {
       int blocks = (int)((total + 7) / 8);
-      if (blocks > 148 * 16) blocks = 148 * 16;
+      if (blocks > sm_count() * 16) blocks = sm_count() * 16;
       gconv_wgrad_reduce_kernel<<<blocks, 256, 0, st>>>(w, ws, KD_pad, dW, db, accumulate,
                                                         bias_done ? 1 : accumulate);
     }

@@ -10,11 +10,10 @@
 
 namespace nlt {
 
-constexpr int kNormSMs = 148;
 
 static inline int norm_grid(size_t n, int block, int per_sm = 8) {
   size_t b = (n + block - 1) / block;
-  const size_t cap = (size_t)kNormSMs * per_sm;
+  const size_t cap = (size_t)sm_count() * per_sm;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;

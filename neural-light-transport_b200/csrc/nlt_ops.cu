@@ -7,11 +7,10 @@
 
 namespace nlt {
 
-constexpr int kSMs = 148;
 
 static inline int grid_for(size_t n, int block, int per_sm = 8) {
   size_t b = (n + block - 1) / block;
-  size_t cap = (size_t)kSMs * per_sm;
+  size_t cap = (size_t)sm_count() * per_sm;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
   return (int)b;

@@ -5,17 +5,17 @@
 // Both are streams of [pixels x K] rows against a tiny [K x 16] matrix (AI ~ 6 FLOP/B), so the design goal is:
 // every input byte crosses HBM once, arrives in shared memory by cp.async (16-byte pieces for float4-able
 // sources, 4-byte pieces for the 3- and 1-channel ones -- no register staging, two tiles in flight), and the math
-// runs as packed FFMA2 (two fp32 FMAs per issued instruction, sm_100) so that the CUDA-core issue rate stays
-// below the HBM time per tile:
+// runs as float2 FMA pairs over (even, odd) channels with constant-bank weights so that the CUDA-core issue rate
+// stays below the HBM time per tile:
 //
 //   tile = 256 consecutive pixels (1x1 conv: each source's tile is one contiguous run of bytes)
 //   smem row of a pixel = [float4-able sources ...][scalar sources ...][zero pad], stride KROW = K4*4 + 4 floats
 //   (an odd number of 16-byte chunks: thread-per-pixel LDS.128 over consecutive rows is bank-conflict free)
 //
 //   forward : thread = pixel, 16 outputs as 16 float2 accumulators over (even, odd) channel pairs; the weight
-//             pairs (W[c][n], W[c+1][n]) sit in shared memory so one broadcast LDS.128 feeds two FFMA2
+//             pairs (W[c][n], W[c+1][n]) sit in constant memory (see pwx_cw)
 //   wgrad   : warp = pixel, lane = (channel quad group cg, output quad ng); dz is staged duplicated
-//             (d, d) so that x pairs (c, c+1) times a broadcast pair accumulate dW[c..c+1][n] in one FFMA2;
+//             (d, d) so that x pairs (c, c+1) times a broadcast pair accumulate dW[c..c+1][n] in one FMA pair;
 //             one fp32 partial per CTA goes to the workspace in the k-group layout of WgradK, the fixed-order
 //             reduce kernel of nlt_gconv.cu finishes (deterministic).
 #include <type_traits>
@@ -24,8 +24,8 @@
 namespace nlt {
 
 // Tile = 128 pixels per CTA of 128 threads, ONE shared-memory stage per CTA (45-51 KB): four to five CTAs share an SM and
-// cover each other's copy latency.  The first version (256-pixel tiles, double-buffered inside one 8-warp CTA per SM)
-// ran at 22 % issue utilisation: eight warps could not hide the LDCU / LDS latency in front of the FFMA2 chains.
+// cover each other's copy latency (one 8-warp CTA per SM with double-buffered 256-pixel tiles could not hide the
+// load latency in front of the FMA chains).
 constexpr int PWX_T = 128;          // pixels per tile
 constexpr int PWX_THREADS = 128;
 constexpr int PWX_WARPS = PWX_THREADS / 32;
@@ -105,10 +105,8 @@ __device__ __forceinline__ void pwx_zero_rows(const PwxParams& p, float* xs, uin
 constexpr int PWX_OROW = 20;        // floats per staged output row (16 + 4: conflict-free STS.128 per pixel)
 
 // The [K x 16] weight matrix lives in CONSTANT memory as (even, odd) channel pairs: every lane of a warp needs the same
-// weight at the same time, so it is fetched by the uniform datapath (LDCU -> uniform registers -> FFMA2 R, R, UR, R)
-// and costs neither an LSU slot nor a shared-memory wavefront.  ncu on the shared-memory version of this kernel
-// (profiles/r2_e_*): 272 broadcast LDS.128 per pixel kept the LSU pipe 58 % busy and the FFMA2s waiting on them
-// (short scoreboard) at 34 % issue utilisation.
+// weight at the same time, so it is a constant-bank operand of the FMA and costs neither an LSU slot nor a
+// shared-memory wavefront (the shared-memory form needed 272 broadcast LDS.128 per pixel).
 constexpr int PWX_CW_PAIRS = 64;                                   // K <= 128
 __constant__ float2 pwx_cw[PWX_CW_PAIRS * 32];                     // [pair][n] = (W[c_even][n], W[c_odd][n]); n < 16 (or 32: d2s form)
 __device__ float2 pwx_cw_stage[PWX_CW_PAIRS * 32];                 // written by the pack kernel, copied into pwx_cw
@@ -123,9 +121,9 @@ __global__ void pwx_pack_w_kernel(const PwxParams p, const float* __restrict__ w
   }
 }
 
-// K4 x NO FFMA2 block of one thread: x row from shared memory, weights [pair][NOUT] from the constant bank at the
-// COMPILE-TIME column offset H * NO (a thread-derived offset, even a warp-uniform one, turns the LDCU operands into
-// per-thread LDC loads: measured 2.7x slower, profiles/r2_t_*)
+// K4 x NO FMA-pair block of one thread: x row from shared memory, weights [pair][NOUT] from the constant bank at the
+// COMPILE-TIME column offset H * NO (a thread-derived offset, even a warp-uniform one, turns the constant-bank operands
+// into per-thread loads)
 template <int K4, int NOUT, int NO, int H>
 __device__ __forceinline__ void pwx_row_mac(const float4* __restrict__ xrow, float2 (&acc)[NO]) {
 #pragma unroll
@@ -136,8 +134,8 @@ __device__ __forceinline__ void pwx_row_mac(const float4* __restrict__ xrow, flo
     const float2 xa = make_float2(xv.x, xv.y), xb = make_float2(xv.z, xv.w);
 #pragma unroll
     for (int n = 0; n < NO; ++n) {
-      acc[n] = __ffma2_rn(xa, pwx_cw[(2 * q) * NOUT + H * NO + n], acc[n]);
-      acc[n] = __ffma2_rn(xb, pwx_cw[(2 * q + 1) * NOUT + H * NO + n], acc[n]);
+      acc[n] = ffma2(xa, pwx_cw[(2 * q) * NOUT + H * NO + n], acc[n]);
+      acc[n] = ffma2(xb, pwx_cw[(2 * q + 1) * NOUT + H * NO + n], acc[n]);
     }
   }
 }
@@ -159,7 +157,6 @@ __device__ __forceinline__ void pwx_row_out(const float2 (&acc)[NO], const float
 
 // NS threads per pixel, each owning 16 / NS outputs (warp-uniform split: the constant-bank weights stay uniform
 // operands); the output stage aliases the x stage, so that the CTA needs 35 KB at K = 64 and 4 CTAs x 8 warps fit.
-// One thread per pixel at 45 KB (the round-2 form until profiles/r2_q_*): 14 resident warps, FMA pipe 51 % busy.
 template <int K4, int NS>
 __global__ void __launch_bounds__(PWX_THREADS * NS, NS == 1 ? (K4 <= 16 ? 6 : (K4 <= 24 ? 4 : 3)) : (K4 <= 16 ? 4 : 3))
 pwx_fwd_kernel(const PwxParams p, const float* __restrict__ bias, const int act, float* __restrict__ out) {
@@ -285,8 +282,8 @@ pwx_wgrad_kernel(const PwxParams p, const float* __restrict__ G, float* __restri
         const float2 xa = make_float2(xv.x, xv.y), xb = make_float2(xv.z, xv.w);
 #pragma unroll
         for (int n = 0; n < 4; ++n) {
-          acc[g][0][n] = __ffma2_rn(xa, gd[n], acc[g][0][n]);
-          acc[g][1][n] = __ffma2_rn(xb, gd[n], acc[g][1][n]);
+          acc[g][0][n] = ffma2(xa, gd[n], acc[g][0][n]);
+          acc[g][1][n] = ffma2(xb, gd[n], acc[g][1][n]);
         }
       }
     }
@@ -418,7 +415,7 @@ static int pwx_fwd_launch(const PwxParams& p, const float* bias, int act, float*
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
   const unsigned per_sm = NS == 1 ? (K4 <= 16 ? 6u : (K4 <= 24 ? 4u : 3u)) : (K4 <= 16 ? 4u : 3u);
-  const unsigned grid = p.ntiles < 148u * per_sm ? p.ntiles : 148u * per_sm;
+  const unsigned grid = p.ntiles < (unsigned)sm_count() * per_sm ? p.ntiles : (unsigned)sm_count() * per_sm;
   pwx_fwd_kernel<K4, NS><<<grid, PWX_THREADS * NS, smem, st>>>(p, bias, act, out);
   NLT_CUDA_LAUNCH_CHECK("pwx_fwd_kernel");
   return NLT_OK;
@@ -437,7 +434,7 @@ int launch_pwx_fwd(const GConvK& k, const float* bias, int act, float* out, cuda
   if (e == cudaSuccess)
     e = cudaMemcpyToSymbolAsync(pwx_cw, stage, (size_t)p.K4 * 2 * 16 * sizeof(float2), 0, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwx weight table: %s", cudaGetErrorString(e));
-  // NLT_PWX_NS: threads per pixel (default 1; 2 = the output split, not faster: profiles/r2_u_*)
+  // NLT_PWX_NS: threads per pixel (default 1; 2 = the output split)
   if (g_opt_pwx_ns < 0) { const char* e = getenv("NLT_PWX_NS"); g_opt_pwx_ns = (e && e[0] == '2') ? 2 : 1; }
   const int ns = g_opt_pwx_ns;
 #define PWX_GO(K4_) do { if (ns == 1) return pwx_fwd_launch<K4_, 1>(p, bias, act, out, smem, st); \
@@ -500,8 +497,8 @@ pwx_d2s_fwd_kernel(const PwxParams p, const float* __restrict__ bias, const int 
       const float2 xa = make_float2(xv.x, xv.y), xb = make_float2(xv.z, xv.w);
 #pragma unroll
       for (int n = 0; n < NOUT; ++n) {
-        acc[n] = __ffma2_rn(xa, pwx_cw[(2 * q) * NOUT + n], acc[n]);
-        acc[n] = __ffma2_rn(xb, pwx_cw[(2 * q + 1) * NOUT + n], acc[n]);
+        acc[n] = ffma2(xa, pwx_cw[(2 * q) * NOUT + n], acc[n]);
+        acc[n] = ffma2(xb, pwx_cw[(2 * q + 1) * NOUT + n], acc[n]);
       }
     }
     __syncthreads();                                           // every row of xs has been read
@@ -583,7 +580,7 @@ static int pwx_d2s_launch(const PwxParams& p, const float* bias, int act, float*
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
   const unsigned per_sm = NOUT == 16 ? 4u : 3u;
-  const unsigned grid = p.ntiles < 148u * per_sm ? p.ntiles : 148u * per_sm;
+  const unsigned grid = p.ntiles < (unsigned)sm_count() * per_sm ? p.ntiles : (unsigned)sm_count() * per_sm;
   pwx_d2s_fwd_kernel<K4, NOUT><<<grid, PWX_THREADS, smem, st>>>(p, bias, act, out, Win);
   NLT_CUDA_LAUNCH_CHECK("pwx_d2s_fwd_kernel");
   return NLT_OK;
@@ -657,8 +654,7 @@ __global__ void pf_pack_w_kernel(const PfParams p, const float* __restrict__ w, 
 
 // NS threads share a pixel, each owning NOUT / NS outputs (the split is warp-uniform, so the constant-bank weights stay
 // uniform operands): twice the resident warps for the same tile, at the price of every x row being read NS times from
-// shared memory.  (ncu of the one-thread-per-pixel form, profiles/r2_q_ncu_full_*: 12 warps/SM, FMA pipe 40 % busy,
-// warps waiting on the LDS.128 of their row.)
+// shared memory.
 template <int K4, int NOUT, int TP, int NS>
 struct PfCfg {
   static constexpr int THR = TP * NS;
@@ -800,11 +796,10 @@ static bool pf_build(const GConvK& k, PfParams* p, int* tp) {
     p->seg_l[s] = sg.C == 4 ? 1 : (sg.C == 8 ? 2 : (sg.C == 16 ? 3 : 4));
     col += 4 * sg.C;
   }
-  // (K = 16 -- the input gradient of the up-conv into 4 channels -- is served better by the wide stencil kernel:
-  //  0.237 vs 0.218 ms on level 12, profiles/r2_r_*)
+  // (K = 16 -- the input gradient of the up-conv into 4 channels -- is left to the wide stencil kernel)
   if (col != 32 && col != 64 && col != 128) return false;
-  // K = 128 into 32 channels needs 64 float2 accumulators next to a 64-pixel tile: 6 warps per SM, measured 3x slower
-  // than the tensor path on level 2 of the 64-channel workload (profiles/r2_p_*)
+  // K = 128 into 32 channels needs 64 float2 accumulators next to a 64-pixel tile: 6 warps per SM; the tensor path
+  // takes it
   if (col == 128 && k.Cout == 32) return false;
   p->nseg = k.nseg; p->K = col;
   *tp = col <= 64 ? 128 : 64;
@@ -838,7 +833,7 @@ static int pf_launch(const PfParams& p, const float* bias, int act, float* out, 
     if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  const unsigned grid = p.ntiles < 148u * per_sm ? p.ntiles : 148u * per_sm;
+  const unsigned grid = p.ntiles < (unsigned)sm_count() * per_sm ? p.ntiles : (unsigned)sm_count() * per_sm;
   pf_fwd_kernel<K4, NOUT, TP, NS><<<grid, TP * NS, smem, st>>>(p, bias, act, out, beta, mask_y, mask_act);
   NLT_CUDA_LAUNCH_CHECK("pf_fwd_kernel");
   return NLT_OK;
@@ -857,7 +852,7 @@ int launch_pf_fwd(const GConvK& k, const float* bias, int act, float beta, const
   if (e == cudaSuccess)
     e = cudaMemcpyToSymbolAsync(pwx_cw, stage, (size_t)(p.K / 2) * k.Cout * sizeof(float2), 0, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwx weight table: %s", cudaGetErrorString(e));
-  // NLT_PF_NS: threads per pixel (default 1; 2 = the output split, measured 0.1-0.2 ms per step slower: profiles/r2_u_*)
+  // NLT_PF_NS: threads per pixel (default 1; 2 = the output split)
   if (g_opt_pf_ns < 0) { const char* e = getenv("NLT_PF_NS"); g_opt_pf_ns = (e && e[0] == '2') ? 2 : 1; }
   const int ns = g_opt_pf_ns;
 #define PF_GO(K4_, N_, TP_) \
@@ -891,7 +886,7 @@ bool pwx_wgrad_applicable(const GConvK& k, const float* G) {
 static size_t pwx_wgrad_smem(const PwxParams& p);
 static unsigned pwx_wgrad_grid(const PwxParams& p) {
   const unsigned per_sm = pwx_wgrad_smem(p) > PWX_SMEM_MAX ? 3u : (unsigned)PWX_CTAS_PER_SM;      // resident CTAs
-  return p.ntiles < 148u * per_sm ? p.ntiles : 148u * per_sm;
+  return p.ntiles < (unsigned)sm_count() * per_sm ? p.ntiles : (unsigned)sm_count() * per_sm;
 }
 
 size_t pwx_wgrad_ws_floats(const GConvK& k) {
@@ -948,7 +943,7 @@ int launch_pwx_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size
 // This is the level-1 / level-2 step of the backward chain and, at 1024^2, the largest single launch group of the
 // whole step.  It is a pure stream (128-256 MB in, 0.5-1 GB out + the read-modify-write operands), so:
 //   * thread = gradient pixel: dz row straight from global memory (a warp reads one contiguous run), the 64 outputs
-//     as 32 float2 accumulators, weights from CONSTANT memory (LDCU + FFMA2, no LSU traffic);
+//     as 32 float2 accumulators, weights from CONSTANT memory (constant-bank FMA operands, no LSU traffic);
 //   * a tile of 256 pixels of one lattice row owns two contiguous 32 KB runs of the output (rows 2y and 2y+1):
 //     results are staged in shared memory and leave as fully coalesced 16-byte stores, with the old gradient
 //     (beta = 1), the activation mask and the fused pointwise term (the final 1x1 conv's input gradient riding along,
@@ -1014,7 +1009,7 @@ pwd2s_kernel(const PwdParams p) {
 #pragma unroll
     for (int q = 0; q < K / 4; ++q) xv[q] = __ldg(xr + q);
   };
-  constexpr bool PREFETCH = K <= 32;                               // K = 64: the 64 extra registers would spill
+  constexpr bool PREFETCH = K * CS <= 512;                         // (K, CS) = (32, 32) / (64, *): the extra registers spill
   float4 xcur[PREFETCH ? K / 4 : 1];
   if (PREFETCH && blockIdx.x < p.ntiles) load_x(blockIdx.x, reinterpret_cast<float4(&)[K / 4]>(xcur));
   for (uint32_t t = blockIdx.x; t < p.ntiles; t += gridDim.x) {
@@ -1025,8 +1020,8 @@ pwd2s_kernel(const PwdParams p) {
 #pragma unroll
     for (int m = 0; m < 32; ++m) acc[m] = make_float2(0.f, 0.f);
     const float4* xrow = reinterpret_cast<const float4*>(p.dz + ((size_t)t * TP + lp) * K);
-    // the tap-row half is warp-uniform, but only a COMPILE-TIME table offset keeps the weights uniform operands
-    // (LDCU -> FFMA2 ..., UR, ...); with `half * 32` as a run-time offset the compiler emitted per-thread LDC loads
+    // the tap-row half is warp-uniform, but only a COMPILE-TIME table offset keeps the weights constant-bank operands;
+    // with `half * 32` as a run-time offset the compiler emits per-thread constant loads
     auto mac = [&](auto hc) {
       constexpr int H = decltype(hc)::value;
 #pragma unroll
@@ -1037,7 +1032,7 @@ pwd2s_kernel(const PwdParams p) {
         for (int e = 0; e < 4; ++e) {
           const float2 xx = make_float2(xs[e], xs[e]);
 #pragma unroll
-          for (int m = 0; m < 32; ++m) acc[m] = __ffma2_rn(xx, pwd_cw[(4 * q + e) * (NP / 2) + H * 32 + m], acc[m]);
+          for (int m = 0; m < 32; ++m) acc[m] = ffma2(xx, pwd_cw[(4 * q + e) * (NP / 2) + H * 32 + m], acc[m]);
         }
       }
     };
@@ -1142,7 +1137,7 @@ static int pwd2s_launch(const PwdParams& p0, cudaStream_t st) {
     if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     if (dev >= 0 && dev < 64) attr_set[dev] = true;
   }
-  const unsigned grid = p.ntiles < 296u ? p.ntiles : 296u;          // 2 CTAs per SM
+  const unsigned grid = p.ntiles < 2u * sm_count() ? p.ntiles : 2u * sm_count();   // 2 CTAs per SM
   pwd2s_kernel<K, CS><<<grid, PWD_THREADS, smem, st>>>(p);
   NLT_CUDA_LAUNCH_CHECK("pwd2s_kernel");
   return NLT_OK;
@@ -1172,7 +1167,7 @@ int launch_pwd2s(const GConvK& k, float beta, const float* mask_y, int mask_act,
 // =============================================================================================
 // Weight gradient of the 2x2 convolutions (stride 1 or 2) of the 16- / 32-channel levels:
 //   dW[tap, c, n] = sum_p x[(s*y + dy, s*x + dx), c] * dz[(y, x), n]     K = 4 * sum_seg C <= 128, N = 16 or 32.
-// Same arithmetic shape as pwx_wgrad_kernel (an outer product per pixel, FFMA2 with the gradient staged duplicated),
+// Same arithmetic shape as pwx_wgrad_kernel (an outer product per pixel, FMA pairs with the gradient staged duplicated),
 // with the pixel's K-vector gathered from a staged input patch: a tile is 64 output pixels of one output row, its
 // input is two row segments per source (s*64 (+1 halo) pixels, contiguous in memory) copied by cp.async.  warp =
 // pixel, lane = (channel group, output quad); for N = 32, K = 128 two warps split the K rows of a pixel.  One fp32
@@ -1289,8 +1284,8 @@ pws_wgrad_kernel(const PwsParams p, const float* __restrict__ G, float* __restri
         const float2 xa = make_float2(xv.x, xv.y), xb = make_float2(xv.z, xv.w);
 #pragma unroll
         for (int nn = 0; nn < 4; ++nn) {
-          acc[j][0][nn] = __ffma2_rn(xa, gd[nn], acc[j][0][nn]);
-          acc[j][1][nn] = __ffma2_rn(xb, gd[nn], acc[j][1][nn]);
+          acc[j][0][nn] = ffma2(xa, gd[nn], acc[j][0][nn]);
+          acc[j][1][nn] = ffma2(xb, gd[nn], acc[j][1][nn]);
         }
       }
     }
@@ -1382,7 +1377,7 @@ static PwsPlan pws_plan(const GConvK& k) {
   const size_t red = ((size_t)PWS_WARPS * (pl.ng * ncg * 4) * k.Cout + PWS_WARPS * k.Cout) * sizeof(float);
   pl.smem = stage > red ? stage : red;
   if (pl.smem > 56 * 1024) return pl;
-  pl.grid = p.ntiles < 148u * PWS_CTAS_PER_SM ? p.ntiles : 148u * PWS_CTAS_PER_SM;
+  pl.grid = p.ntiles < (unsigned)sm_count() * PWS_CTAS_PER_SM ? p.ntiles : (unsigned)sm_count() * PWS_CTAS_PER_SM;
   pl.ok = true;
   return pl;
 }

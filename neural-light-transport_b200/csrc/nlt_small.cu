@@ -17,7 +17,6 @@
 
 namespace nlt {
 
-constexpr int kSMs = 148;
 
 // -----------------------------------------------------------------------------
 // pointwise conv
@@ -43,10 +42,9 @@ bool pw_conv_applicable(const GConvK& k) {
 
 // One thread = one pixel x QT consecutive quads of GEMM columns (QT*4 outputs), R pixels in flight.
 // QT = 4 means a thread owns 16 output channels of a pixel: every input value is loaded once per 64 FMAs
-// and the thread stores 64 contiguous bytes (ncu showed the QT = 1 form issue-bound: ~14 overhead
-// instructions per FMA).
-// 4 CTAs per SM (64 registers, a few spilled words outside the k loop): the kernel is latency-bound, and
-// measured 3-8 % faster per launch than the 2-3 CTAs the unconstrained allocation (90+ registers) allows.
+// and the thread stores 64 contiguous bytes (the QT = 1 form is issue-bound: ~14 overhead instructions per FMA).
+// 4 CTAs per SM (64 registers, a few spilled words outside the k loop): the kernel is latency-bound and wants the
+// occupancy more than the registers of the unconstrained allocation (90+).
 //
 // EX: a second, pointwise term on the OUTPUT lattice is added in the epilogue,
 //   out[pix, c] += sum_k ex.x[pix, k] * ex.w[k * wk + c * wn]        (k < ex.K <= PW_EX_KMAX)
@@ -344,7 +342,7 @@ int launch_pw_conv(const GConvK& k, const float* bias, int act, float beta, cons
   else if (nq <= 4) pw_launch<4, 4, 2>(k, bias, act, beta, mask_y, mask_act, out, ex, st);
   else if (nq <= 8) pw_launch<8, 4, 2>(k, bias, act, beta, mask_y, mask_act, out, ex, st);
   // fused term: one pixel per thread -- at 64 registers the two-pixel form spills ~130 bytes per thread and
-  // the local-memory traffic exceeded the useful traffic (ncu: profiles/r1_k_ncu_full_pw_kernels.csv)
+  // the local-memory traffic exceeded the useful traffic
   else if (ex != nullptr) pw_launch<16, 4, 1>(k, bias, act, beta, mask_y, mask_act, out, ex, st);
   else pw_launch<16, 4, 2>(k, bias, act, beta, mask_y, mask_act, out, ex, st);
   NLT_CUDA_LAUNCH_CHECK("pw_conv_kernel");
@@ -533,16 +531,15 @@ dconv_small_kernel(const GConvK g, const float* __restrict__ bias, const int act
 // -----------------------------------------------------------------------------
 // Wide form of the small direct convolution: one thread = one lattice pixel x ALL 16 output channels (4
 // quads), R pixels per thread.  For the 16 -> 16 channel stencils (K = taps * C = 64) the tiled implicit-GEMM
-// kernel spends ~64 % of its instructions on address generation (ncu source view, profiles/r1_i); here every
+// kernel spends most of its instructions on address generation; here every
 // input float4 is loaded once per 64 FMAs and every weight LDS.128 feeds 4*R FMAs.  Vector sources only, no
 // depth-to-space (those go to the pointwise kernel).
 // -----------------------------------------------------------------------------
 constexpr int DW_KMAX = 128;   // taps * channels of the widest routed stencil (32 -> 32 channels, 2x2)
 
 // CW = true: the weight table [k][quad] lives in CONSTANT memory (filled per launch by dconv_cw_pack_kernel + a
-// device-to-device symbol copy).  Every lane needs the same weight at the same time, so it arrives through the uniform
-// datapath (LDCU -> uniform registers) and the FMAs are issued as packed FFMA2 with a uniform operand: neither the
-// 128 broadcast LDS.128 per pixel of the shared-memory form nor half of its FMA instructions are issued.
+// device-to-device symbol copy).  Every lane needs the same weight at the same time, so it is a constant-bank operand
+// of the FMA: the 128 broadcast LDS.128 per pixel of the shared-memory form are not issued.
 // One table per device: launches from different streams must not overlap (the engine issues forward convs and input
 // gradients from its main stream only; weight gradients, on the side stream, never use this kernel).
 __constant__ float4 dw_cw[DW_KMAX * 8];
@@ -657,8 +654,8 @@ dconv_wide_kernel(const GConvK g, const float* __restrict__ bias, const int act,
 #pragma unroll
                 for (int r = 0; r < R; ++r) {
                   const float2 aa = make_float2(a[r][kk], a[r][kk]);
-                  const float2 lo = __ffma2_rn(aa, make_float2(w.x, w.y), make_float2(acc[r][j][0], acc[r][j][1]));
-                  const float2 hi = __ffma2_rn(aa, make_float2(w.z, w.w), make_float2(acc[r][j][2], acc[r][j][3]));
+                  const float2 lo = ffma2(aa, make_float2(w.x, w.y), make_float2(acc[r][j][0], acc[r][j][1]));
+                  const float2 hi = ffma2(aa, make_float2(w.z, w.w), make_float2(acc[r][j][2], acc[r][j][3]));
                   acc[r][j][0] = lo.x; acc[r][j][1] = lo.y; acc[r][j][2] = hi.x; acc[r][j][3] = hi.y;
                 }
               } else {
@@ -735,7 +732,7 @@ static bool dconv_wide_common(const GConvK& k, const float* out, const float* ma
   return aligned16(out) && (mask_y == nullptr || aligned16(mask_y));
 }
 
-int g_opt_dconv_wide8 = -1;    // the 8-output form (up-conv levels 11-12); default on (validated in round 2: profiles/r2_a_*)
+int g_opt_dconv_wide8 = -1;    // the 8-output form (up-conv levels 11-12); default on
 
 bool dconv_wide_applicable(const GConvK& k, const float* out, const float* mask_y) {
   if (g_opt_dconv_wide < 0) {
@@ -755,7 +752,7 @@ bool dconv_wide_applicable(const GConvK& k, const float* out, const float* mask_
   return g_opt_dconv_wide8 > 0 && dconv_wide_common(k, out, mask_y, 8, DW_KMAX, true);
 }
 
-int g_opt_dconv_cw = -1;   // option "dconv_cw" / NLT_DCONV_CW: constant-memory weight table + FFMA2 (default on)
+int g_opt_dconv_cw = -1;   // option "dconv_cw" / NLT_DCONV_CW: constant-memory weight table (default on)
 
 static int dconv_cw_fill(const GConvK& k, int qt, cudaStream_t st) {
   dconv_cw_pack_kernel<<<8, 256, 0, st>>>(k, qt);
@@ -859,7 +856,7 @@ static bool ws_plan(const GConvK& k, WsPlan& pl) {
   pl.p = p;
   pl.ld = pl.nq * 4;
   pl.KD_pad = (size_t)(p * pl.kq + 1) * 4;
-  long long want = (long long)kSMs * (p <= 2 ? 8 : 4);
+  long long want = (long long)sm_count() * (p <= 2 ? 8 : 4);
   const long long max_split = ((long long)k.M + 255) / 256;
   if (want > max_split) want = max_split;
   if (want < 1) want = 1;
@@ -1021,7 +1018,7 @@ wgrad_small_kernel(const WgradK w, const float* __restrict__ G, float* __restric
 }
 
 // -----------------------------------------------------------------------------
-// Row-run form of the warp-stream wgrad.  ncu on wgrad_small_kernel<4,2,4>: ~170 warp instructions per
+// Row-run form of the warp-stream wgrad.  wgrad_small_kernel<4,2,4> issues ~170 warp instructions per
 // pixel for 36 FMAs -- the flat pixel index is decoded and every source address rebuilt from scratch for
 // every pixel.  Here a warp owns a run of WR_CHUNK consecutive lattice pixels of one row: (n, ty) and all
 // base pointers are set up once per run and the pixel loop only adds constant strides.  Requires float4
@@ -1347,13 +1344,13 @@ static TppPlan tpp_plan(const GConvK& k) {
   pl.k.rows = pl.KG * 4;
   pl.k.ldw = (k.Cout + 3) / 4 * 4;
   pl.k.bias_row = (pl.KG - 1) * 4;
-  long long want = (long long)kSMs * 6;
+  long long want = (long long)sm_count() * 6;
   const long long max_split = ((long long)k.M + TPP_THREADS * 4 - 1) / (TPP_THREADS * 4);
   if (want > max_split) want = max_split;
   if (want < 1) want = 1;
   pl.nsplit = (int)want;
   // the 9-load tile (final conv: 36 channels -> 3) needs ~190 registers = 8 warps per SM; three blocks of 3
-  // loads each run at 4x the occupancy and re-read only the 3-channel gradient (measured in profiles/r1_j)
+  // loads each run at 4x the occupancy and re-read only the 3-channel gradient
   pl.ksplit = (pl.vec == 4 && pl.n == 3 && nl == 9) ? 3 : 1;
   pl.ok = true;
   return pl;
@@ -1404,7 +1401,7 @@ int launch_wgrad_small(const GConvK& k, const float* G, float* ws, WgradK* w, si
   const bool rows = g_opt_wgrad_rows == 1 && wgrad_rows_ok(k, G);
   const uint32_t cpr = ((uint32_t)k.ax.nt + WR_CHUNK - 1) / WR_CHUNK;
   const uint32_t nchunks = (uint32_t)k.N * (uint32_t)k.ay.nt * cpr;
-  // measured on B200 (profiles/r1_h): P <= 2 wants occupancy (128 registers, 4 CTAs per SM), the wide
+  // P <= 2 wants occupancy (128 registers, 4 CTAs per SM), the wide
   // P >= 4 tiles want more pixels in flight instead (they spill below ~220 registers)
 #define NLT_WS(NQ_, P_)                                                                                        \
   do {                                                                                                         \

@@ -1,23 +1,24 @@
-// tcgen05 tensor-core path of the generalised convolution (sm_100a only).
+// wgmma tensor-core path of the generalised convolution (sm_90a).
 //
-// Implicit GEMM  D[128 pixels x BN] += A[128 pixels x 32 ch] * B[32 ch x BN]  per K-block, where a
-// K-block is (tap, segment, 32-channel chunk).  No im2col: for every tap the A tile is ONE TMA box of the
-// NHWC activation tensor, [TH x TW pixels] x [32 channels], landing in shared memory as 128 rows of 128 B with
-// the 128-byte swizzle -- exactly the K-major operand layout tcgen05.mma consumes.  SAME padding is TMA
-// out-of-bounds zero fill (coordinates may be negative); the k == stride "patch" conv is a 5-D view of the
-// same tensor (c, dx, x/s, dy, n*H/s + y/s) so that no element stride is needed.
+// Implicit GEMM  D[128 pixels x BN] += A[128 pixels x KBW ch] * B[KBW ch x BN]  per K-block, where a K-block is
+// (tap, segment, KBW-channel chunk).  No im2col: for every tap the A tile is ONE TMA box of the NHWC activation
+// tensor, [TH x TW pixels] x [KBW channels], landing in shared memory as 128 rows of 128 B (KBW = 32, 128-byte
+// swizzle) or 64 B (KBW = 16, 64-byte swizzle) -- the K-major operand layout wgmma reads.  SAME padding is TMA
+// out-of-bounds zero fill (coordinates may be negative); the k == stride "patch" conv is a 5-D view of the same
+// tensor (c, dx, x/s, dy, n*H/s + y/s) so that no element stride is needed.
 //
-// fp32-class accuracy on TF32 tensor cores: 3xTF32.  Weights are split once per call into hi/lo TF32
-// planes (pack kernel); activations are split in shared memory by four transform warps
-// (hi = rna_tf32(a) in place, lo = rna_tf32(a - hi) in a second buffer) and the MMA warp issues
-// D += Ahi*Bhi + Ahi*Blo + Alo*Bhi with fp32 accumulation in TMEM.
+// fp32-class accuracy on TF32 tensor cores: 3xTF32.  Weights are split once per call into hi/lo TF32 planes (pack
+// kernel); activations are split by the consumer warpgroups (hi = x truncated or rounded to TF32, lo = x - hi
+// rounded to TF32) and every 8-channel k-step issues D += Alo*Bhi + Ahi*Blo + Ahi*Bhi with fp32 accumulation in
+// registers.
 //
-// Warp roles (320 threads, 1 CTA / SM, persistent over output tiles):
-//   warp 0      TMA producer      (A raw tile + Bhi + Blo per stage, mbarrier complete_tx)
-//   warp 1      MMA issuer        (single thread; tcgen05.commit frees stages / publishes accumulators)
-//   warps 2-5   operand transform (smem -> smem split, fence.proxy.async)
-//   warps 6-9   epilogue          (tcgen05.ld -> bias / activation / beta / derivative mask -> global)
-// Accumulators are double-buffered in TMEM so the epilogue of tile t overlaps the MMAs of tile t+1.
+// Warp roles (384 threads, 1 CTA / SM, persistent over output tiles):
+//   warpgroup 0      warp 0, one thread: TMA producer (A raw tile + Bhi + Blo per stage, mbarrier complete_tx)
+//   warpgroups 1-2   consumers of rows [0, 64) / [64, 128) of the tile: operand split, wgmma m64nBNk8, epilogue
+// The producer runs ahead into the next tile's stages while the consumers drain their accumulators.
+// Two forms of the A operand (option "tcs"): RS = fragments read from the raw tile and split in registers (wgmma
+// with A in registers, nothing written back to shared memory); SS = the consumer warpgroup writes hi / lo planes
+// of its 64 rows into shared memory (wgmma with both operands in shared memory).
 #include <cuda.h>
 #include "nlt_common.cuh"
 
@@ -25,11 +26,9 @@ namespace nlt {
 
 constexpr int TC_MAX_STAGES = 8;                // smem ring depth is chosen per shape (2..8): bytes in flight, not math, bound most layers
 constexpr int TC_BM = 128;
-// channels per K-block: 32 (128-byte rows, SWIZZLE_128B) or 16 (64-byte rows, SWIZZLE_64B)
-constexpr int TC_EPI_PAD = 36;                  // floats per staging row (32 columns + 4 pad: conflict-free)
-constexpr int TC_EPI_BYTES = 4 * 32 * TC_EPI_PAD * 4;   // epilogue staging: 4 warps x 32 rows
-constexpr int TC_THREADS = 320;               // wgrad kernel: TMA + MMA + 8 transform warps (4 of them double as epilogue)
-constexpr int TCF_THREADS = 448;              // forward kernel: TMA + MMA + 4 transform + 4 epilogue + 4 more transform warps
+constexpr int TC_EPI_PAD = 36;                  // floats per staging row (32 columns + 4 pad)
+constexpr int TC_EPI_BYTES = 8 * 16 * TC_EPI_PAD * 4;   // epilogue staging: 8 consumer warps x 16 rows
+constexpr int TC_THREADS = 384;                 // producer warpgroup + two consumer warpgroups (both kernels)
 constexpr uint32_t TC_SPIN_LIMIT = 1u << 28;    // watchdog: trap instead of hanging the GPU
 unsigned long long g_tc_launches = 0;           // tensor-core kernel launches (diagnostic)
 
@@ -55,14 +54,12 @@ struct TcParams {
   int Hout, Wout, cout_true, Cout;   // Cout = GEMM columns (d2s: s*s*cout_true)
   int o0y, osy, o0x, osx;            // output pixel = o0 + os * lattice coordinate (non-d2s)
   int d2s, d2s_s;
-  // exact multiply-shift division by the run-time tile / channel counts: the per-tile coordinate decode of the producer
-  // and the per-pass address arithmetic of the epilogue warps were chains of 32-bit integer divisions (~150 cycles
-  // each); with everything else ablated a tile still cost 4 us (profiles/r2_z_*)
+  // exact multiply-shift division by the run-time tile / channel counts (per-tile coordinate decode of the producer,
+  // per-pass address arithmetic of the epilogue): no 32-bit integer division on the critical path of a tile
   FastDiv div_ntn, div_tpi, div_tx, div_tw, div_ct, div_s;
   int act, mask_act;
   int stages;               // smem ring depth
-  int rawhi;                // option "tc_rawhi" / NLT_TC_RAWHI (default 1): A-hi operand = the raw fp32 tile (no hi plane write)
-  int ablate;               // DIAGNOSTIC (NLT_TC_ABLATE, wrong results!): 1 no B loads, 2 no transform, 4 no MMA, 8 no epilogue memory traffic, 16 no A loads
+  int rawhi;                // option "tc_rawhi" / NLT_TC_RAWHI (default 1): A-hi = x truncated to TF32 (0: rounded)
   float beta;
   const float* bias;
   const float* mask_y;
@@ -92,28 +89,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
   return ok != 0;
 }
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  return ok != 0;
-}
-// DIAGNOSTIC switch (NLT_TC_ABLATE bit 32): poll with the non-suspending test_wait instead of try_wait
-__device__ int g_tc_poll = 0;
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
-  if (g_tc_poll) {
-    while (!mbar_test_wait(bar, parity)) {
-      if (++spins > TC_SPIN_LIMIT) { asm volatile("trap;"); }
-    }
-    return;
-  }
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > TC_SPIN_LIMIT) { asm volatile("trap;"); }
   }
+}
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
   asm volatile(
@@ -132,74 +116,110 @@ __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+// ---- wgmma (m64nNk8, TF32 inputs, fp32 accumulators in registers) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int NR>
+__device__ __forceinline__ void acc_fence(float (&d)[NR]) {
+#pragma unroll
+  for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D[tmem] (+)= A[smem] * B[smem], TF32 inputs, fp32 accumulate, M=128
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+// D (+)= A * B; scale_d == 0 overwrites D.  SS: A and B from shared-memory descriptors; RS: A from registers
+// (per warp a 16 x 8 slice: a[0] = (g, t), a[1] = (g + 8, t), a[2] = (g, t + 4), a[3] = (g + 8, t + 4), g = lane / 4,
+// t = lane % 4).  D: d[4j + 2h + e] = (row g + 8h, column 8j + 2t + e) of the warp's 16 rows.
+__device__ __forceinline__ void wgmma_ss(float (&d)[8], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+__device__ __forceinline__ void wgmma_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
 }
-// TS form: A operand in tensor memory (see nlt_tcts.cu for the probe of the layout this relies on)
-__device__ __forceinline__ void tc_mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
+__device__ __forceinline__ void wgmma_ss(float (&d)[16], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accum) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&r)[16]) {
+__device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tc_st8(uint32_t taddr, const uint32_t (&r)[8]) {
+__device__ __forceinline__ void wgmma_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, int scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
 }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
+}
+
+// K-major swizzled operand tile: rows of ROWB bytes (128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B), 8-row core matrices.
+// Stepping K by 8 TF32 values inside the swizzle atom advances the start address by 32 bytes.
+template <int ROWB>
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address
+  d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)((8 * ROWB) >> 4) << 32;             // stride byte offset: 8 rows
+  d |= (uint64_t)(ROWB == 128 ? 1 : 2) << 62;         // SWIZZLE_128B / SWIZZLE_64B
+  return d;
+}
 
 __device__ __forceinline__ float tf32_rna(float x) {
   uint32_t r;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
-// Round-to-nearest TF32 in two integer instructions (cvt.rna.tf32 expands to ~8 SASS instructions with its
-// inf/nan handling; ncu showed the operand split bound by exactly that).  Adding half an ulp to the bit
-// pattern and clearing the low 13 mantissa bits rounds the magnitude to nearest (ties away), carries into
-// the exponent correctly, and is only wrong for inf/nan, which the split does not need to preserve.
+// Round-to-nearest TF32 in two integer instructions (cvt.rna.tf32 expands to several instructions with its inf/nan
+// handling).  Adding half an ulp to the bit pattern and clearing the low 13 mantissa bits rounds the magnitude to
+// nearest (ties away), carries into the exponent correctly, and is only wrong for inf/nan, which the split does not
+// need to preserve.
 __device__ __forceinline__ float tf32_round(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-// K-major swizzled operand tile: rows of ROWB bytes (128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B), 8-row atoms.
-template <int ROWB>
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address
-  d |= (uint64_t)1 << 16;                             // leading byte offset (unused for swizzled K-major) = 16 B
-  d |= (uint64_t)((8 * ROWB) >> 4) << 32;             // stride byte offset: 8 rows
-  d |= (uint64_t)1 << 46;                             // descriptor version (Blackwell)
-  d |= (uint64_t)(ROWB == 128 ? 2 : 4) << 61;         // SWIZZLE_128B / SWIZZLE_64B
-  return d;
+// 3xTF32 split of one activation: hi = x truncated (rawhi) or rounded to TF32; lo = x - hi (exact), rounded to TF32
+__device__ __forceinline__ void tf32_split(float x, int rawhi, uint32_t& hi, uint32_t& lo) {
+  const float h = rawhi ? __uint_as_float(__float_as_uint(x) & 0xFFFFE000u) : tf32_round(x);
+  hi = __float_as_uint(h);
+  lo = __float_as_uint(tf32_round(x - h));
 }
 
 // ---------------------------------------------------------------------------------------------
-// weight pack: Bhi/Blo [kb][Cout_pad][32] (K-major rows of 128 B), TF32-rounded split
+// weight pack: Bhi/Blo [kb][Cout_pad][KBW] (K-major rows), TF32-rounded split
 // ---------------------------------------------------------------------------------------------
 __global__ void tc_pack_weights_kernel(const GConvK g, int kbw, int kb_total, int chunks_per_tap, int cout_pad,
                                        float* __restrict__ bhi, float* __restrict__ blo) {
@@ -234,66 +254,48 @@ struct TcMaps {
   CUtensorMap bhi, blo;
 };
 
-template <int BN, int KBW>
-__global__ void __launch_bounds__(TCF_THREADS, 1)
+template <int BN, int KBW, bool RS>
+__global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gconv_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
   constexpr int ROWB = KBW * 4;                   // bytes per operand row
-  constexpr int TC_KB = KBW;
-  constexpr int TC_A_BYTES = TC_BM * ROWB;
+  constexpr int KS = KBW / 8;                     // k-steps per K-block
+  constexpr int A_BYTES = TC_BM * ROWB;
+  constexpr int A_HALF = 64 * ROWB;               // one consumer warpgroup's rows
   constexpr int B_BYTES = BN * ROWB;
-  constexpr int STAGE_BYTES = 2 * TC_A_BYTES + 2 * B_BYTES;
-  constexpr uint32_t TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
+  constexpr int A_PLANES = RS ? 1 : 2;            // raw tile (RS) / hi + lo planes (SS)
+  constexpr int STAGE_BYTES = A_PLANES * A_BYTES + 2 * B_BYTES;
 
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle
   // offset arithmetic on the __shared__ array keeps the address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t bars[3 * TC_MAX_STAGES + 4];
-  const int TC_STAGES = p.stages;
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t bars[2 * TC_MAX_STAGES];
+  const int S = p.stages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t bar0 = smem_u32(bars);
   auto bar_full = [&](int s) { return bar0 + 8u * s; };
-  auto bar_ready = [&](int s) { return bar0 + 8u * (TC_MAX_STAGES + s); };
-  auto bar_empty = [&](int s) { return bar0 + 8u * (2 * TC_MAX_STAGES + s); };
-  auto bar_accf = [&](int b) { return bar0 + 8u * (3 * TC_MAX_STAGES + b); };
-  auto bar_acce = [&](int b) { return bar0 + 8u * (3 * TC_MAX_STAGES + 2 + b); };
+  auto bar_empty = [&](int s) { return bar0 + 8u * (TC_MAX_STAGES + s); };
   const uint32_t smem_base = smem_u32(smem);
   auto a_hi = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES; };
-  auto a_lo = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + TC_A_BYTES; };
-  auto b_hi = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + 2 * TC_A_BYTES; };
-  auto b_lo = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + 2 * TC_A_BYTES + B_BYTES; };
+  auto b_hi = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + A_PLANES * A_BYTES; };
+  auto b_lo = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + A_PLANES * A_BYTES + B_BYTES; };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
+    for (int s = 0; s < S; ++s) {
       mbar_init(bar_full(s), 1);
-      mbar_init(bar_ready(s), 8);                  // one arrival per transform warp (see the transform role)
-      mbar_init(bar_empty(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_accf(b), 1);
-      mbar_init(bar_acce(b), 4);                   // one arrival per epilogue warp
+      mbar_init(bar_empty(s), 8);                  // one arrival per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)),
-                 "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
   const int kb_total = p.kb_total;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
@@ -309,505 +311,196 @@ tc_gconv_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
             for (int s = 0; s < p.nseg; ++s)
               for (int ch = 0; ch < p.seg_chunks[s]; ++ch, ++kb) {
                 mbar_wait(bar_empty(stage), phase ^ 1);
-                mbar_expect_tx(bar_full(stage), ((p.ablate & 16) ? 0 : TC_A_BYTES) + ((p.ablate & 1) ? 0 : 2 * B_BYTES));
-                if (!(p.ablate & 16)) {
-                  if (p.mode_patch)
-                    tma_load_5d(a_hi(stage), &maps.a[s], bar_full(stage), ch * TC_KB, ux, tx0, uy, n * p.Hs + ty0);
-                  else
-                    tma_load_4d(a_hi(stage), &maps.a[s], bar_full(stage), ch * TC_KB, tx0 + ux * p.ux_step + p.x_off,
-                                ty0 + uy * p.uy_step + p.y_off, n);
-                }
-                if (!(p.ablate & 1)) {
-                  tma_load_3d(b_hi(stage), &maps.bhi, bar_full(stage), 0, nt * BN, kb);
-                  tma_load_3d(b_lo(stage), &maps.blo, bar_full(stage), 0, nt * BN, kb);
-                }
-                if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-              }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int buf = it & 1;
-        const uint32_t acc_phase = (uint32_t)(it >> 1) & 1;
-        mbar_wait(bar_acce(buf), acc_phase ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(bar_ready(stage), phase);        // operands split and visible to the async proxy
-          tc_fence_after();
-#pragma unroll
-          for (int k = 0; k < ((p.ablate & 4) ? 0 : TC_KB / 8); ++k) {
-            const uint64_t ah = umma_desc_kmajor<ROWB>(a_hi(stage) + k * 32), al = umma_desc_kmajor<ROWB>(a_lo(stage) + k * 32);
-            const uint64_t bh = umma_desc_kmajor<ROWB>(b_hi(stage) + k * 32), bl = umma_desc_kmajor<ROWB>(b_lo(stage) + k * 32);
-            tc_mma_tf32(d_tmem, al, bh, IDESC, (kb | k) != 0);   // small terms first
-            tc_mma_tf32(d_tmem, ah, bl, IDESC, 1);
-            tc_mma_tf32(d_tmem, ah, bh, IDESC, 1);
-          }
-          tc_commit(bar_empty(stage));               // stage reusable once these MMAs have read it
-          if (kb == kb_total - 1) tc_commit(bar_accf(buf));
-          if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp < 6 || warp >= 10) {
-    // ================= operand transform: fp32 -> (hi, lo) TF32 planes (warps 2-5 and 10-13) =================
-    // eight warps: with four, one warp per scheduler ran this dependent LDS -> cvt -> STS chain at ~0.3 IPC
-    const int t = warp < 6 ? threadIdx.x - 64 : threadIdx.x - 320 + 128;   // 0..255
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      for (int kb = 0; kb < kb_total; ++kb) {
-        mbar_wait(bar_full(stage), phase);
-        float4* ah = reinterpret_cast<float4*>(smem + (size_t)stage * STAGE_BYTES);
-        float4* al = reinterpret_cast<float4*>(smem + (size_t)stage * STAGE_BYTES + TC_A_BYTES);
-#pragma unroll
-        for (int i = 0; i < ((p.ablate & 2) ? 0 : TC_A_BYTES / 16 / 256); ++i) {
-          const int q = t + i * 256;              // physical 16-byte chunk: elementwise, swizzle-agnostic
-          const float4 v = ah[q];
-          float4 h, l;
-          if (p.rawhi) {
-            // the tensor core reads the upper 19 bits of an fp32 word (measured: tests/test_gpu_tcts.py): the raw tile IS
-            // the hi operand, only lo = x - trunc(x) (exact in fp32, then rounded to TF32) has to be written
-            h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u); h.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-            h.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u); h.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-            l.x = tf32_round(v.x - h.x); l.y = tf32_round(v.y - h.y); l.z = tf32_round(v.z - h.z); l.w = tf32_round(v.w - h.w);
-            al[q] = l;
-          } else {
-            h.x = tf32_round(v.x); h.y = tf32_round(v.y); h.z = tf32_round(v.z); h.w = tf32_round(v.w);
-            l.x = tf32_round(v.x - h.x); l.y = tf32_round(v.y - h.y); l.z = tf32_round(v.z - h.z); l.w = tf32_round(v.w - h.w);
-            ah[q] = h;
-            al[q] = l;
-          }
-        }
-        // every thread makes its writes visible to the async proxy; ONE arrival per warp: 256 single-thread arrivals
-        // on the same mbarrier word serialise (they were the largest part of the kernel's per-k-block fixed cost)
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_ready(stage));
-        if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else {
-    // ================= epilogue =================
-    // TMEM -> registers (lane = pixel) -> bias/activation -> per-warp smem staging -> transposed read
-    // (8 lanes = 128 contiguous bytes of one pixel) -> beta / derivative-mask -> coalesced global store.
-    // The read-modify-write operands of the NEXT 32-column chunk are loaded before the current one is
-    // processed, so their DRAM latency overlaps the TMEM drain.
-    const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32)
-    float* stg = reinterpret_cast<float*>(smem + (size_t)TC_STAGES * STAGE_BYTES) + quarter * 32 * TC_EPI_PAD;
-    const bool rmw = ((p.beta != 0.f) || (p.mask_y != nullptr)) && !(p.ablate & 8);
-    constexpr int NCH = (BN + 31) / 32;           // 32-column chunks per tile (BN == 16: one half-used chunk)
-    constexpr int CW = BN < 32 ? BN : 32;         // columns per chunk
-    constexpr int QPR = CW / 4;                   // float4 quads per pixel row of a chunk
-    constexpr int RPI = 32 / QPR;                 // pixel rows covered per pass of the warp
-    constexpr int NPASS = 32 / RPI;               // passes per chunk (== QPR)
-    const int lq = lane % QPR, lr = lane / QPR;
-
-    // Output addressing without per-pass arithmetic: offset(tile, pass i, column) = tile base + row_off[i] + col_off, where
-    // row_off depends only on the lane (computed once per kernel) and col_off only on (column tile, chunk).  The
-    // epilogue warps are the busiest role of this kernel on the many-tile levels (ncu source view, profiles/r2_af_*:
-    // ~85 % of their samples are not waits) -- every instruction here is on the critical path of a tile.
-    const int sxy = p.d2s ? p.d2s_s : 1;
-    int row_off[NPASS];
-#pragma unroll
-    for (int i = 0; i < NPASS; ++i) {
-      const int row = quarter * 32 + i * RPI + lr;
-      const int rty = (int)fdiv((uint32_t)row, p.div_tw), rtx = row - rty * p.TW;
-      row_off[i] = p.d2s ? (rty * sxy * p.Wout + rtx * sxy) * p.cout_true
-                         : (p.osy * rty * p.Wout + p.osx * rtx) * p.cout_true;
-    }
-    auto tile_base = [&](int tile, int& nt) -> size_t {
-      const int mt = (int)fdiv((uint32_t)tile, p.div_ntn);
-      nt = tile - mt * p.n_tiles_n;
-      const int n = (int)fdiv((uint32_t)mt, p.div_tpi);
-      const int r = mt - n * tiles_per_img;
-      const int rq = (int)fdiv((uint32_t)r, p.div_tx);
-      const int ty0 = rq * p.TH, tx0 = (r - rq * p.tiles_x) * p.TW;
-      const int oy = p.d2s ? ty0 * sxy : p.o0y + p.osy * ty0, ox = p.d2s ? tx0 * sxy : p.o0x + p.osx * tx0;
-      return (((size_t)n * p.Hout + oy) * p.Wout + ox) * p.cout_true;
-    };
-    // offset of GEMM column nb inside an output pixel group (d2s: which of the s x s pixels, which channel)
-    auto col_off = [&](int nb) -> int {
-      if (!p.d2s) return nb;
-      const int tap = (int)fdiv((uint32_t)nb, p.div_ct);
-      const int dy = (int)fdiv((uint32_t)tap, p.div_s);
-      return (dy * p.Wout + (tap - dy * p.d2s_s)) * p.cout_true + (nb - tap * p.cout_true);
-    };
-    const bool bias_vec = p.bias != nullptr && aligned16(p.bias);
-    const int act = p.act;
-    const float neg = act == NLT_ACT_LEAKYRELU ? 0.3f : (act == NLT_ACT_RELU ? 0.f : 1.f);
-    float4 rm_old[NPASS], rm_y[NPASS];
-    auto prefetch = [&](size_t base) {
-#pragma unroll
-      for (int i = 0; i < NPASS; ++i) {
-        const size_t ob = base + (size_t)row_off[i];
-        rm_old[i] = (p.beta != 0.f) ? *reinterpret_cast<const float4*>(p.out + ob) : make_float4(0.f, 0.f, 0.f, 0.f);
-        rm_y[i] = (p.mask_y != nullptr) ? ld4(p.mask_y + ob) : make_float4(1.f, 1.f, 1.f, 1.f);
-      }
-    };
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1;
-      int nt;
-      const size_t tbase = tile_base(tile, nt);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN);
-#pragma unroll 1
-      for (int ch = 0; ch < NCH; ++ch) {
-        const int col0 = nt * BN + ch * 32;       // GEMM column of this chunk
-        const size_t cbase = tbase + (size_t)col_off(col0 + lq * 4);
-        // read-modify-write operands first: their latency overlaps the accumulator wait / TMEM drain
-        if (rmw) prefetch(cbase);
-        if (ch == 0) {
-          mbar_wait(bar_accf(buf), acc_phase);
-          tc_fence_after();
-        }
-#pragma unroll
-        for (int h = 0; h < CW / 16; ++h) {
-          uint32_t v[16];
-          tc_ld16(taddr + ch * 32 + h * 16, v);
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            int cb = col0 + h * 16 + q4 * 4;
-            if (p.d2s) cb -= (int)fdiv((uint32_t)cb, p.div_ct) * p.cout_true;
-            float4 bq = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (bias_vec) bq = ld4(p.bias + cb);
-            else if (p.bias != nullptr) bq = make_float4(__ldg(p.bias + cb), __ldg(p.bias + cb + 1), __ldg(p.bias + cb + 2), __ldg(p.bias + cb + 3));
-            float o[4] = {__uint_as_float(v[q4 * 4 + 0]) + bq.x, __uint_as_float(v[q4 * 4 + 1]) + bq.y,
-                          __uint_as_float(v[q4 * 4 + 2]) + bq.z, __uint_as_float(v[q4 * 4 + 3]) + bq.w};
-            if (act == NLT_ACT_ELU) {             // warp-uniform
-#pragma unroll
-              for (int e = 0; e < 4; ++e) o[e] = elu_slow(o[e]);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 4; ++e) o[e] = o[e] > 0.f ? o[e] : neg * o[e];
-            }
-            *reinterpret_cast<float4*>(stg + lane * TC_EPI_PAD + h * 16 + q4 * 4) = make_float4(o[0], o[1], o[2], o[3]);
-          }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < NPASS; ++i) {
-          const int row = i * RPI + lr;
-          float4 o = *reinterpret_cast<const float4*>(stg + row * TC_EPI_PAD + lq * 4);
-          if (rmw) {
-            o.x += p.beta * rm_old[i].x; o.y += p.beta * rm_old[i].y; o.z += p.beta * rm_old[i].z; o.w += p.beta * rm_old[i].w;
-            if (p.mask_y != nullptr) {
-              o.x *= act_bwd_from_y(rm_y[i].x, p.mask_act); o.y *= act_bwd_from_y(rm_y[i].y, p.mask_act);
-              o.z *= act_bwd_from_y(rm_y[i].z, p.mask_act); o.w *= act_bwd_from_y(rm_y[i].w, p.mask_act);
-            }
-          }
-          const size_t ob = cbase + (size_t)row_off[i];
-          if (!(p.ablate & 8) || o.x == 123456.f) *reinterpret_cast<float4*>(p.out + ob) = o;
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_acce(buf));
-    }
-  }
-
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-  }
-}
-
-template <int BN, int KBW>
-__global__ void __launch_bounds__(TCF_THREADS, 1)
-tcs_gconv_kernel(const __grid_constant__ TcMaps maps, const TcParams p) {
-  constexpr int ROWB = KBW * 4;                   // bytes per operand row
-  constexpr int TC_KB = KBW;
-  constexpr int TC_A_BYTES = TC_BM * ROWB;
-  constexpr int B_BYTES = BN * ROWB;
-  constexpr int STAGE_BYTES = TC_A_BYTES + 2 * B_BYTES;          // raw A tile + Bhi + Blo (no A-lo plane: A goes to TMEM)
-  constexpr int NTA = (512 - 2 * BN) / (2 * KBW) < 8 ? (512 - 2 * BN) / (2 * KBW) : 8;   // TMEM stages of the A operand
-  constexpr uint32_t ACOL0 = 2 * BN;                             // first A column (behind the two accumulators)
-  constexpr uint32_t TMEM_NEED = ACOL0 + NTA * 2 * KBW;
-  constexpr uint32_t TMEM_COLS = TMEM_NEED <= 64 ? 64 : TMEM_NEED <= 128 ? 128 : TMEM_NEED <= 256 ? 256 : 512;
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment for the 128B swizzle
-  // offset arithmetic on the __shared__ array keeps the address space (LDS/STS instead of generic LD/ST)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t bars[4 * TC_MAX_STAGES + 4];
-  const int TC_STAGES = p.stages;
-  __shared__ uint32_t tmem_base_smem;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t bar0 = smem_u32(bars);
-  auto bar_full = [&](int s) { return bar0 + 8u * s; };                              // TMA -> converters / MMA (smem stage)
-  auto bar_empty = [&](int s) { return bar0 + 8u * (TC_MAX_STAGES + s); };           // converters (256) + MMA commit (1) -> TMA
-  auto bar_aready = [&](int t) { return bar0 + 8u * (2 * TC_MAX_STAGES + t); };      // converters -> MMA (TMEM stage)
-  auto bar_afree = [&](int t) { return bar0 + 8u * (3 * TC_MAX_STAGES + t); };       // MMA commit -> converters
-  auto bar_accf = [&](int b) { return bar0 + 8u * (4 * TC_MAX_STAGES + b); };
-  auto bar_acce = [&](int b) { return bar0 + 8u * (4 * TC_MAX_STAGES + 2 + b); };
-  const uint32_t smem_base = smem_u32(smem);
-  auto a_hi = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES; };          // the raw fp32 A tile
-  auto b_hi = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + TC_A_BYTES; };
-  auto b_lo = [&](int s) { return smem_base + (uint32_t)s * STAGE_BYTES + TC_A_BYTES + B_BYTES; };
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < TC_STAGES; ++s) {
-      mbar_init(bar_full(s), 1);
-      mbar_init(bar_empty(s), 257);
-    }
-    for (int t = 0; t < NTA; ++t) {
-      mbar_init(bar_aready(t), 256);
-      mbar_init(bar_afree(t), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_accf(b), 1);
-      mbar_init(bar_acce(b), 128);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)),
-                 "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  const int kb_total = p.kb_total;
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-
-  if (warp == 0) {
-    // ================= TMA producer =================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int mt = (int)fdiv((uint32_t)tile, p.div_ntn);
-        const int nt = tile - mt * p.n_tiles_n;
-        const int n = (int)fdiv((uint32_t)mt, p.div_tpi);
-        const int r = mt - n * tiles_per_img;
-        const int rq = (int)fdiv((uint32_t)r, p.div_tx);
-        const int ty0 = rq * p.TH, tx0 = (r - rq * p.tiles_x) * p.TW;
-        int kb = 0;
-        for (int uy = 0; uy < p.ntap_y; ++uy)
-          for (int ux = 0; ux < p.ntap_x; ++ux)
-            for (int s = 0; s < p.nseg; ++s)
-              for (int ch = 0; ch < p.seg_chunks[s]; ++ch, ++kb) {
-                mbar_wait(bar_empty(stage), phase ^ 1);
-                mbar_expect_tx(bar_full(stage), TC_A_BYTES + 2 * B_BYTES);   // raw A + Bhi + Blo
+                mbar_expect_tx(bar_full(stage), A_BYTES + 2 * B_BYTES);
                 if (p.mode_patch)
-                  tma_load_5d(a_hi(stage), &maps.a[s], bar_full(stage), ch * TC_KB, ux, tx0, uy, n * p.Hs + ty0);
+                  tma_load_5d(a_hi(stage), &maps.a[s], bar_full(stage), ch * KBW, ux, tx0, uy, n * p.Hs + ty0);
                 else
-                  tma_load_4d(a_hi(stage), &maps.a[s], bar_full(stage), ch * TC_KB, tx0 + ux * p.ux_step + p.x_off,
+                  tma_load_4d(a_hi(stage), &maps.a[s], bar_full(stage), ch * KBW, tx0 + ux * p.ux_step + p.x_off,
                               ty0 + uy * p.uy_step + p.y_off, n);
                 tma_load_3d(b_hi(stage), &maps.bhi, bar_full(stage), 0, nt * BN, kb);
                 tma_load_3d(b_lo(stage), &maps.blo, bar_full(stage), 0, nt * BN, kb);
-                if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
+                if (++stage == S) { stage = 0; phase ^= 1; }
               }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      int stage = 0, ts = 0;
-      uint32_t phase = 0, tphase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int buf = it & 1;
-        const uint32_t acc_phase = (uint32_t)(it >> 1) & 1;
-        mbar_wait(bar_acce(buf), acc_phase ^ 1);     // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-        for (int kb = 0; kb < kb_total; ++kb) {
-          mbar_wait(bar_full(stage), phase);         // B planes of this stage have landed
-          mbar_wait(bar_aready(ts), tphase);         // A (hi, lo) of this k-block is in tensor memory
-          tc_fence_after();
-          const uint32_t a_col = tmem_base + ACOL0 + (uint32_t)(ts * 2 * KBW);
-#pragma unroll
-          for (int k = 0; k < TC_KB / 8; ++k) {
-            const uint64_t bh = umma_desc_kmajor<ROWB>(b_hi(stage) + k * 32), bl = umma_desc_kmajor<ROWB>(b_lo(stage) + k * 32);
-            tc_mma_tf32_ts(d_tmem, a_col + KBW + 8 * k, bh, IDESC, (kb | k) != 0);   // Alo * Bhi   (small terms first)
-            tc_mma_tf32_ts(d_tmem, a_col + 8 * k, bl, IDESC, 1);                     // Ahi * Blo
-            tc_mma_tf32_ts(d_tmem, a_col + 8 * k, bh, IDESC, 1);                     // Ahi * Bhi
-          }
-          tc_commit(bar_empty(stage));               // B planes of the smem stage are free once these MMAs have read them
-          tc_commit(bar_afree(ts));                  // ... and so is the TMEM stage
-          if (kb == kb_total - 1) tc_commit(bar_accf(buf));
-          if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-          if (++ts == NTA) { ts = 0; tphase ^= 1; }
-        }
-      }
-    }
-  } else if (warp < 6 || warp >= 10) {
-    // ================= operand conversion: raw fp32 rows in shared memory -> (hi, lo) TF32 columns in TMEM =================
-    // thread = pixel row = TMEM lane (a warp may only touch the lane quarter warp % 4); two warps per quarter share
-    // the KBW channels of a k-block.  One conflict-free LDS.128 per four channels (the TMA swizzle is undone in the
-    // address), the split in registers, tcgen05.st -- no smem -> smem pass, no A-lo plane, no proxy fence.
-    const int quarter = warp & 3, half = warp >= 10 ? 1 : 0;
-    const int r = quarter * 32 + lane;
-    constexpr int CH = KBW / 2;                      // channels per thread and k-block
-    const uint32_t lane_base = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    int stage = 0, ts = 0;
-    uint32_t phase = 0, tphase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      for (int kb = 0; kb < kb_total; ++kb) {
-        mbar_wait(bar_full(stage), phase);
-        const uint8_t* row = smem + (size_t)stage * STAGE_BYTES + (size_t)r * ROWB;
-        float4 v[CH / 4];
-#pragma unroll
-        for (int i = 0; i < CH / 4; ++i) {
-          const int c = half * (CH / 4) + i;        // logical 16-byte chunk of the row
-          const int pc = ROWB == 128 ? (c ^ (r & 7)) : (c ^ ((r >> 1) & 3));
-          v[i] = *reinterpret_cast<const float4*>(row + pc * 16);
-        }
-        uint32_t hi[CH], lo[CH];
-#pragma unroll
-        for (int i = 0; i < CH / 4; ++i) {
-          const float x[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            // the tensor core TRUNCATES a 32-bit TF32 operand to its upper 19 bits (measured: tests/test_gpu_tcts.py,
-            // profiles/r2_c_tcts_probe.json), so the raw fp32 word IS the hi part; lo = x - trunc(x) is exact in
-            // fp32 and is rounded to TF32 so that the dominant residual stays unbiased
-            const uint32_t xb = __float_as_uint(x[e]);
-            hi[4 * i + e] = xb;
-            lo[4 * i + e] = __float_as_uint(tf32_round(x[e] - __uint_as_float(xb & 0xFFFFE000u)));
-          }
-        }
-        mbar_wait(bar_afree(ts), tphase ^ 1);        // the MMAs that read this TMEM stage last time are done
-        tc_fence_after();
-        const uint32_t a_col = lane_base + ACOL0 + (uint32_t)(ts * 2 * KBW) + (uint32_t)(half * CH);
-        if constexpr (CH == 16) { tc_st16(a_col, hi); tc_st16(a_col + KBW, lo); }
-        else { tc_st8(a_col, hi); tc_st8(a_col + KBW, lo); }
-        tc_wait_st();
-        tc_fence_before();
-        mbar_arrive(bar_aready(ts));
-        mbar_arrive(bar_empty(stage));               // this thread is done reading the raw tile
-        if (++stage == TC_STAGES) { stage = 0; phase ^= 1; }
-        if (++ts == NTA) { ts = 0; tphase ^= 1; }
-      }
-    }
-  } else {
-    // ================= epilogue =================
-    // TMEM -> registers (lane = pixel) -> bias/activation -> per-warp smem staging -> transposed read
-    // (8 lanes = 128 contiguous bytes of one pixel) -> beta / derivative-mask -> coalesced global store.
-    // The read-modify-write operands of the NEXT 32-column chunk are loaded before the current one is
-    // processed, so their DRAM latency overlaps the TMEM drain.
-    const int quarter = warp & 3;                 // TMEM lanes [32*quarter, +32)
-    float* stg = reinterpret_cast<float*>(smem + (size_t)TC_STAGES * STAGE_BYTES) + quarter * 32 * TC_EPI_PAD;
-    const bool rmw = (p.beta != 0.f) || (p.mask_y != nullptr);
-    constexpr int NCH = (BN + 31) / 32;           // 32-column chunks per tile (BN == 16: one half-used chunk)
-    constexpr int CW = BN < 32 ? BN : 32;         // columns per chunk
-    constexpr int QPR = CW / 4;                   // float4 quads per pixel row of a chunk
-    constexpr int RPI = 32 / QPR;                 // pixel rows covered per pass of the warp
-    constexpr int NPASS = 32 / RPI;               // passes per chunk (== QPR)
-    const int lq = lane % QPR, lr = lane / QPR;
-
-    struct Coord { int n, ty0, tx0, nt; };
-    auto tile_coord = [&](int tile) {
-      Coord c;
-      const int mt = (int)fdiv((uint32_t)tile, p.div_ntn);
-      c.nt = tile - mt * p.n_tiles_n;
-      c.n = (int)fdiv((uint32_t)mt, p.div_tpi);
-      const int r = mt - c.n * tiles_per_img;
-      const int rq = (int)fdiv((uint32_t)r, p.div_tx);
-      c.ty0 = rq * p.TH; c.tx0 = (r - rq * p.tiles_x) * p.TW;
-      return c;
-    };
-    // element offset of (tile row, GEMM column) in the output tensor
-    auto out_off = [&](const Coord& c, int row, int nb) -> size_t {
-      const int rty = (int)fdiv((uint32_t)row, p.div_tw);
-      const int ty = c.ty0 + rty, tx = c.tx0 + row - rty * p.TW;
-      int cb = nb, oy, ox;
-      if (p.d2s) {
-        const int tap = (int)fdiv((uint32_t)nb, p.div_ct);
-        cb = nb - tap * p.cout_true;
-        const int dy = (int)fdiv((uint32_t)tap, p.div_s);
-        oy = ty * p.d2s_s + dy; ox = tx * p.d2s_s + (tap - dy * p.d2s_s);
-      } else {
-        oy = p.o0y + p.osy * ty; ox = p.o0x + p.osx * tx;
-      }
-      return (((size_t)c.n * p.Hout + oy) * p.Wout + ox) * p.cout_true + cb;
-    };
-    float4 rm_old[NPASS], rm_y[NPASS];
-    auto prefetch = [&](const Coord& c, int ch) {
-#pragma unroll
-      for (int i = 0; i < NPASS; ++i) {
-        const size_t ob = out_off(c, quarter * 32 + i * RPI + lr, c.nt * BN + ch * 32 + lq * 4);
-        rm_old[i] = (p.beta != 0.f) ? *reinterpret_cast<const float4*>(p.out + ob) : make_float4(0.f, 0.f, 0.f, 0.f);
-        rm_y[i] = (p.mask_y != nullptr) ? ld4(p.mask_y + ob) : make_float4(1.f, 1.f, 1.f, 1.f);
-      }
-    };
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1;
-      const Coord tc = tile_coord(tile);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN);
-#pragma unroll 1
-      for (int ch = 0; ch < NCH; ++ch) {
-        // read-modify-write operands first: their latency overlaps the accumulator wait / TMEM drain
-        if (rmw) prefetch(tc, ch);
-        if (ch == 0) {
-          mbar_wait(bar_accf(buf), acc_phase);
-          tc_fence_after();
-        }
-        const int col0 = tc.nt * BN + ch * 32;    // GEMM column of this chunk
-#pragma unroll
-        for (int h = 0; h < CW / 16; ++h) {
-          uint32_t v[16];
-          tc_ld16(taddr + ch * 32 + h * 16, v);
-#pragma unroll
-          for (int q4 = 0; q4 < 4; ++q4) {
-            int cb = col0 + h * 16 + q4 * 4;
-            if (p.d2s) cb -= (int)fdiv((uint32_t)cb, p.div_ct) * p.cout_true;
-            float o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              float x = __uint_as_float(v[q4 * 4 + e]);
-              if (p.bias != nullptr) x += __ldg(p.bias + cb + e);
-              o[e] = act_fwd(x, p.act);
-            }
-            *reinterpret_cast<float4*>(stg + lane * TC_EPI_PAD + h * 16 + q4 * 4) = make_float4(o[0], o[1], o[2], o[3]);
-          }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < NPASS; ++i) {
-          const int row = i * RPI + lr;
-          float4 o = *reinterpret_cast<const float4*>(stg + row * TC_EPI_PAD + lq * 4);
-          if (rmw) {
-            o.x += p.beta * rm_old[i].x; o.y += p.beta * rm_old[i].y; o.z += p.beta * rm_old[i].z; o.w += p.beta * rm_old[i].w;
-            if (p.mask_y != nullptr) {
-              o.x *= act_bwd_from_y(rm_y[i].x, p.mask_act); o.y *= act_bwd_from_y(rm_y[i].y, p.mask_act);
-              o.z *= act_bwd_from_y(rm_y[i].z, p.mask_act); o.w *= act_bwd_from_y(rm_y[i].w, p.mask_act);
-            }
-          }
-          const size_t ob = out_off(tc, quarter * 32 + row, col0 + lq * 4);
-          *reinterpret_cast<float4*>(p.out + ob) = o;
-        }
-        __syncwarp();
-      }
-      tc_fence_before();
-      mbar_arrive(bar_acce(buf));
-    }
+    return;
   }
 
-  // ---- teardown ----
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
+  // ================= consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64) =================
+  const int wg = (warp >> 2) - 1;
+  const int wq = warp & 3;                        // warp inside the warpgroup: rows [64 wg + 16 wq, +16)
+  const int g = lane >> 2, t = lane & 3;
+  const int r0 = 64 * wg + 16 * wq + g;           // this thread's accumulator rows: r0, r0 + 8
+  // RS: physical 16-byte chunk of logical chunk c in rows r0 / r0 + 8 (the same for both: TMA swizzle by row)
+  auto swz = [&](int c) { return ROWB == 128 ? (c ^ (r0 & 7)) : (c ^ ((r0 >> 1) & 3)); };
+
+  // epilogue geometry: accumulator -> bias / activation -> per-warp smem staging [16 rows x 32 columns] -> transposed
+  // read (QPR lanes = one pixel's contiguous columns) -> beta / derivative mask -> coalesced float4 stores
+  float* stg = reinterpret_cast<float*>(smem + (size_t)S * STAGE_BYTES) + (warp - 4) * 16 * TC_EPI_PAD;
+  const bool rmw = (p.beta != 0.f) || (p.mask_y != nullptr);
+  constexpr int NCH = (BN + 31) / 32;             // 32-column chunks per tile (BN == 16: one half-used chunk)
+  constexpr int CW = BN < 32 ? BN : 32;           // columns per chunk
+  constexpr int QPR = CW / 4;                     // float4 quads per pixel row of a chunk
+  constexpr int RPI = 32 / QPR;                   // pixel rows covered per pass of the warp
+  constexpr int NPASS = 16 / RPI;                 // passes per chunk
+  const int lq = lane % QPR, lr = lane / QPR;
+  // output offset(tile, pass i, column) = tile base + row_off[i] + col_off(column): row_off depends only on the lane
+  const int sxy = p.d2s ? p.d2s_s : 1;
+  int row_off[NPASS], row_y[NPASS], row_x[NPASS];   // row_y / row_x: the pass's pixel inside the tile
+#pragma unroll
+  for (int i = 0; i < NPASS; ++i) {
+    const int row = 64 * wg + 16 * wq + i * RPI + lr;
+    const int rty = (int)fdiv((uint32_t)row, p.div_tw), rtx = row - rty * p.TW;
+    row_y[i] = rty; row_x[i] = rtx;
+    row_off[i] = p.d2s ? (rty * sxy * p.Wout + rtx * sxy) * p.cout_true
+                       : (p.osy * rty * p.Wout + p.osx * rtx) * p.cout_true;
+  }
+  // tile origin -> output offset of its first pixel; rem_y / rem_x: lattice rows / columns left from the origin (the
+  // last tiles of a lattice that is not a multiple of the tile shape are partly outside it)
+  auto tile_base = [&](int tile, int& nt, int& rem_y, int& rem_x) -> size_t {
+    const int mt = (int)fdiv((uint32_t)tile, p.div_ntn);
+    nt = tile - mt * p.n_tiles_n;
+    const int n = (int)fdiv((uint32_t)mt, p.div_tpi);
+    const int r = mt - n * tiles_per_img;
+    const int rq = (int)fdiv((uint32_t)r, p.div_tx);
+    const int ty0 = rq * p.TH, tx0 = (r - rq * p.tiles_x) * p.TW;
+    rem_y = p.Hl - ty0; rem_x = p.Wl - tx0;
+    const int oy = p.d2s ? ty0 * sxy : p.o0y + p.osy * ty0, ox = p.d2s ? tx0 * sxy : p.o0x + p.osx * tx0;
+    return (((size_t)n * p.Hout + oy) * p.Wout + ox) * p.cout_true;
+  };
+  // offset of GEMM column nb inside an output pixel group (d2s: which of the s x s pixels, which channel)
+  auto col_off = [&](int nb) -> int {
+    if (!p.d2s) return nb;
+    const int tap = (int)fdiv((uint32_t)nb, p.div_ct);
+    const int dy = (int)fdiv((uint32_t)tap, p.div_s);
+    return (dy * p.Wout + (tap - dy * p.d2s_s)) * p.cout_true + (nb - tap * p.cout_true);
+  };
+  const int act = p.act;
+  const float neg = act == NLT_ACT_LEAKYRELU ? 0.3f : (act == NLT_ACT_RELU ? 0.f : 1.f);
+
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    for (int kb = 0; kb < kb_total; ++kb) {
+      mbar_wait(bar_full(stage), phase);
+      const uint32_t bh0 = b_hi(stage), bl0 = b_lo(stage);
+      if constexpr (RS) {
+        const uint8_t* at = smem + (size_t)stage * STAGE_BYTES + (size_t)r0 * ROWB + t * 4;
+        uint32_t ah[KS][4], al[KS][4];
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float x = *reinterpret_cast<const float*>(at + (e & 1) * 8 * ROWB + swz(2 * ks + (e >> 1)) * 16);
+            tf32_split(x, p.rawhi, ah[ks][e], al[ks][e]);
+          }
+        acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          const uint64_t bh = wgmma_desc<ROWB>(bh0 + ks * 32), bl = wgmma_desc<ROWB>(bl0 + ks * 32);
+          wgmma_rs(acc, al[ks], bh, (kb | ks) != 0);   // small terms first
+          wgmma_rs(acc, ah[ks], bl, 1);
+          wgmma_rs(acc, ah[ks], bh, 1);
+        }
+      } else {
+        // split this warpgroup's 64 rows: the raw tile becomes the hi plane in place, lo goes to the second plane
+        // (elementwise over physical 16-byte chunks: swizzle-agnostic)
+        float4* ah = reinterpret_cast<float4*>(smem + (size_t)stage * STAGE_BYTES + wg * A_HALF);
+        float4* al = reinterpret_cast<float4*>(smem + (size_t)stage * STAGE_BYTES + A_BYTES + wg * A_HALF);
+        const int tw = threadIdx.x - 128 - 128 * wg;
+#pragma unroll
+        for (int i = 0; i < A_HALF / 16 / 128; ++i) {
+          const int q = tw + i * 128;
+          const float4 v = ah[q];
+          uint32_t h[4], l[4];
+          tf32_split(v.x, p.rawhi, h[0], l[0]); tf32_split(v.y, p.rawhi, h[1], l[1]);
+          tf32_split(v.z, p.rawhi, h[2], l[2]); tf32_split(v.w, p.rawhi, h[3], l[3]);
+          ah[q] = make_float4(__uint_as_float(h[0]), __uint_as_float(h[1]), __uint_as_float(h[2]), __uint_as_float(h[3]));
+          al[q] = make_float4(__uint_as_float(l[0]), __uint_as_float(l[1]), __uint_as_float(l[2]), __uint_as_float(l[3]));
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
+        named_bar_sync(1 + wg, 128);
+        const uint32_t ahi0 = a_hi(stage) + wg * A_HALF, alo0 = ahi0 + A_BYTES;
+        acc_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < KS; ++ks) {
+          const uint64_t dah = wgmma_desc<ROWB>(ahi0 + ks * 32), dal = wgmma_desc<ROWB>(alo0 + ks * 32);
+          const uint64_t bh = wgmma_desc<ROWB>(bh0 + ks * 32), bl = wgmma_desc<ROWB>(bl0 + ks * 32);
+          wgmma_ss(acc, dal, bh, (kb | ks) != 0);      // small terms first
+          wgmma_ss(acc, dah, bl, 1);
+          wgmma_ss(acc, dah, bh, 1);
+        }
+      }
+      wgmma_commit();
+      // wait for this K-block's MMAs before the next one: in the RS form the next split writes the registers these
+      // MMAs still read (keeping one group in flight would need a second fragment set and 32 more registers per
+      // thread at BN = 128); the TMA ring and the other warpgroup cover the wait
+      wgmma_wait_all();
+      acc_fence(acc);
+      // the stage is free once this warp's MMAs have read it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty(stage));
+      if (++stage == S) { stage = 0; phase ^= 1; }
+    }
+
+    // ================= epilogue =================
+    int nt, rem_y, rem_x;
+    const size_t tbase = tile_base(tile, nt, rem_y, rem_x);
+    bool valid[NPASS];
+#pragma unroll
+    for (int i = 0; i < NPASS; ++i) valid[i] = row_y[i] < rem_y && row_x[i] < rem_x;
+#pragma unroll
+    for (int ch = 0; ch < NCH; ++ch) {
+      const int col0 = nt * BN + ch * 32;         // GEMM column of this chunk
+      const size_t cbase = tbase + (size_t)col_off(col0 + lq * 4);
+      float4 rm_old[NPASS], rm_y[NPASS];
+      if (rmw) {                                  // read-modify-write operands first: their latency overlaps the staging
+#pragma unroll
+        for (int i = 0; i < NPASS; ++i) {
+          const size_t ob = cbase + (size_t)row_off[i];
+          rm_old[i] = (p.beta != 0.f && valid[i]) ? *reinterpret_cast<const float4*>(p.out + ob) : make_float4(0.f, 0.f, 0.f, 0.f);
+          rm_y[i] = (p.mask_y != nullptr && valid[i]) ? ld4(p.mask_y + ob) : make_float4(1.f, 1.f, 1.f, 1.f);
+        }
+      }
+#pragma unroll
+      for (int jj = 0; jj < CW / 8; ++jj) {
+        const int j = ch * 4 + jj;                // 8-column group of the accumulator
+        int cb = col0 + jj * 8 + 2 * t;
+        if (p.d2s) cb -= (int)fdiv((uint32_t)cb, p.div_ct) * p.cout_true;
+        float b0 = 0.f, b1 = 0.f;
+        if (p.bias != nullptr) { b0 = __ldg(p.bias + cb); b1 = __ldg(p.bias + cb + 1); }
+        float o[4] = {acc[4 * j] + b0, acc[4 * j + 1] + b1, acc[4 * j + 2] + b0, acc[4 * j + 3] + b1};
+        if (act == NLT_ACT_ELU) {                 // warp-uniform
+#pragma unroll
+          for (int e = 0; e < 4; ++e) o[e] = elu_slow(o[e]);
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) o[e] = o[e] > 0.f ? o[e] : neg * o[e];
+        }
+        *reinterpret_cast<float2*>(stg + g * TC_EPI_PAD + jj * 8 + 2 * t) = make_float2(o[0], o[1]);
+        *reinterpret_cast<float2*>(stg + (g + 8) * TC_EPI_PAD + jj * 8 + 2 * t) = make_float2(o[2], o[3]);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < NPASS; ++i) {
+        const int row = i * RPI + lr;
+        float4 o = *reinterpret_cast<const float4*>(stg + row * TC_EPI_PAD + lq * 4);
+        if (rmw) {
+          o.x += p.beta * rm_old[i].x; o.y += p.beta * rm_old[i].y; o.z += p.beta * rm_old[i].z; o.w += p.beta * rm_old[i].w;
+          if (p.mask_y != nullptr) {
+            o.x *= act_bwd_from_y(rm_y[i].x, p.mask_act); o.y *= act_bwd_from_y(rm_y[i].y, p.mask_act);
+            o.z *= act_bwd_from_y(rm_y[i].z, p.mask_act); o.w *= act_bwd_from_y(rm_y[i].w, p.mask_act);
+          }
+        }
+        if (valid[i]) *reinterpret_cast<float4*>(p.out + cbase + (size_t)row_off[i]) = o;
+      }
+      __syncwarp();
+    }
   }
 }
 
@@ -834,7 +527,7 @@ static EncodeTiledFn get_encode() {
 
 struct TcPlan {
   bool ok;
-  bool ts;      // TS form (tcs_gconv_kernel)
+  bool ts;      // RS form of the A operand (option tcs)
   int bn;
   int kbw;
   TcParams p;
@@ -852,13 +545,13 @@ static int pick_bn(int cout) {
   return 0;
 }
 
-// "tcs" (TS form: A operand converted on the way into tensor memory, tcs_gconv_kernel): option / NLT_TCS,
-// 1 = use it wherever the tensor path applies (and from NLT_TCS_KMIN contraction terms on), 0 = SS form only
+// option "tc" = 2 (A/B testing): every shape the kernel can run takes it, ignoring the size heuristics below
+int g_tc_force = 0;
+
+// "tcs" (option / NLT_TCS): 1 = RS form (A operand split in registers), 0 = SS form (hi / lo planes in shared memory)
 int g_opt_tcs = -1;
-static int g_tcs_kmin = -1;
 static bool tcs_enabled() {
   if (g_opt_tcs < 0) { const char* e = getenv("NLT_TCS"); g_opt_tcs = e ? (atoi(e) != 0) : NLT_TCS_DEFAULT; }
-  if (g_tcs_kmin < 0) { const char* e = getenv("NLT_TCS_KMIN"); g_tcs_kmin = e ? atoi(e) : 64; }
   return g_opt_tcs == 1;
 }
 
@@ -882,27 +575,26 @@ static TcPlan tc_plan(const GConvK& k) {
   }
   const int TC_KB = pl.kbw;
   if (!aligned16(k.w)) { /* weights are only read by the pack kernel: no alignment needed */ }
-  if (ts) {
-    if (k.ay.nu * k.ax.nu * ctot < g_tcs_kmin) return pl;
-  } else {
+  if (!g_tc_force) {
     // with less than 64 contraction terms the op is a pure stream: the pointwise / fp32 kernels are faster there
     if (k.ay.nu * k.ax.nu * ctot < 64) return pl;
-    // measured: 16-channel (64-byte-row) K-blocks only pay off from K = 128 up
+    // 16-channel (64-byte-row) K-blocks only from K = 128 up: below that the FFMA stream kernels take these layers
     if (pl.kbw == 16 && k.ay.nu * k.ax.nu * ctot < 128) return pl;
   }
   if (k.ay.nu < 1 || k.ax.nu < 1) return pl;
   TcParams& p = pl.p;
   p.N = k.N; p.Hl = k.ay.nt; p.Wl = k.ax.nt;
   // tile shape
-  if (p.Wl >= TC_BM) {
-    if (p.Wl % TC_BM) return pl;
-    p.TW = TC_BM; p.TH = 1;
-  } else {
-    if (TC_BM % p.Wl) return pl;
-    p.TW = p.Wl; p.TH = TC_BM / p.Wl;
-    if (p.Hl % p.TH) return pl;
-  }
-  p.tiles_x = p.Wl / p.TW; p.tiles_y = p.Hl / p.TH;
+  // tile shape: TW = 128 lattice columns, or the smallest power of two >= Wl; partial tiles at the right / bottom
+  // edge load zeros (TMA out-of-bounds fill) or rows that only feed masked outputs, and store nothing outside.
+  // Only option tc = 2 takes lattices that are not a multiple of the tile shape: at the 1x1 .. 4x4 bottleneck levels
+  // most rows of a tile would be masked, and the fp32 kernels serve those layers
+  if (p.Hl < 1 || p.Wl < 1) return pl;
+  p.TW = TC_BM;
+  while (p.TW / 2 >= p.Wl) p.TW /= 2;
+  p.TH = TC_BM / p.TW;
+  if (!g_tc_force && (p.Wl % p.TW != 0 || p.Hl % p.TH != 0)) return pl;
+  p.tiles_x = (p.Wl + p.TW - 1) / p.TW; p.tiles_y = (p.Hl + p.TH - 1) / p.TH;
   // coordinate map
   const bool stride1 = (k.ay.it == 1 && k.ax.it == 1);
   const bool patch = (!k.d2s && k.ay.it > 1 && k.ay.it == k.ax.it && k.ay.iu == 1 && k.ax.iu == 1 && k.ay.i0 == 0 &&
@@ -921,14 +613,14 @@ static TcPlan tc_plan(const GConvK& k) {
   p.Hout = k.Hout; p.Wout = k.Wout; p.cout_true = k.cout_true; p.Cout = k.Cout;
   p.o0y = k.ay.o0; p.osy = k.ay.os; p.o0x = k.ax.o0; p.osx = k.ax.os;
   p.d2s = k.d2s; p.d2s_s = k.d2s_s;
-  // few output tiles: narrower column tiles so that more SMs get work (A is re-read from L2)
-  // (only while the finer tiling still fits ONE wave of 148 CTAs: every tile pays the ~10 us pipeline fill / drain of
-  // the kernel again, profiles/r2_i_tc_ablation_31.txt; NLT_TC_SPLIT_WAVES=1 restores the round-1 rule "< 148 tiles")
+  // few output tiles: narrower column tiles so that more SMs get work (A is re-read from L2), but only while the finer
+  // tiling still fits ONE wave of persistent CTAs: every tile pays the pipeline fill / drain of the kernel again
+  // (NLT_TC_SPLIT_WAVES=1: split whenever there are fewer tiles than SMs)
   static int split_waves = -1;
   if (split_waves < 0) { const char* e = getenv("NLT_TC_SPLIT_WAVES"); split_waves = (e && e[0] == '1') ? 1 : 0; }
   while (pl.bn > 32) {
     const long long tiles = (long long)p.N * p.tiles_x * p.tiles_y * (k.Cout / pl.bn);
-    if (split_waves ? tiles >= 148 : 2 * tiles > 148) break;
+    if (split_waves ? tiles >= sm_count() : 2 * tiles > sm_count()) break;
     pl.bn /= 2;
   }
   p.n_tiles_n = k.Cout / pl.bn;
@@ -949,17 +641,8 @@ static TcPlan tc_plan(const GConvK& k) {
     pl.smem_bytes = (size_t)st * stage_bytes + TC_EPI_BYTES + 1024;
   }
   if (get_encode() == nullptr) return pl;
-  {
-    static int ablate = -1;
-    if (ablate < 0) {
-      const char* e = getenv("NLT_TC_ABLATE");
-      ablate = e ? atoi(e) : 0;
-      if (ablate & 32) { const int one = 1; cudaMemcpyToSymbol(g_tc_poll, &one, sizeof(int)); }
-    }
-    p.ablate = ablate;
-    if (g_opt_tc_rawhi < 0) { const char* e = getenv("NLT_TC_RAWHI"); g_opt_tc_rawhi = (e && e[0] == '0') ? 0 : 1; }
-    p.rawhi = g_opt_tc_rawhi;
-  }
+  if (g_opt_tc_rawhi < 0) { const char* e = getenv("NLT_TC_RAWHI"); g_opt_tc_rawhi = (e && e[0] == '0') ? 0 : 1; }
+  p.rawhi = g_opt_tc_rawhi;
   pl.ok = true;
   return pl;
 }
@@ -1009,16 +692,15 @@ static int encode_maps(const GConvK& k, const TcPlan& pl, const float* bhi, cons
 }
 
 // =============================================================================================
-// tcgen05 weight gradient:  dW[Kd x N] = sum_p A[p, Kd]^T * G[p, N]   (3xTF32, fp32 accumulate in TMEM)
+// wgmma weight gradient:  dW[Kd x N] = sum_p A[p, Kd]^T * G[p, N]   (3xTF32, fp32 accumulate in registers)
 //
-// The contraction runs over PIXELS.  tf32 tensor-core operands must be K-major here (the only MN-major
-// tf32 layout, 128B_ATOM_32B, needs 32-channel rows and would exclude the 16-channel layers that own most
-// of the bytes), so the four transform warps TRANSPOSE while they split: TMA brings raw [32 pixels x w
-// channels] pieces (w <= 32, hardware-swizzled so the transposing reads are bank-conflict free), the
-// transform writes hi/lo planes [channel row][32 pixels = 128 B] in the K-major SWIZZLE_128B layout, and
-// the MMA warp issues 4 K-steps x 3 products per 32-pixel stage into ONE [128 x BN] accumulator that lives
-// in TMEM for the CTA's whole pixel range.  Works for any channel counts that are multiples of 4.
-// The bias gradient (column sums of G) is accumulated by the transform warps on the way.  One fp32
+// The contraction runs over PIXELS.  TF32 wgmma operands must be K-major, so the two consumer warpgroups
+// TRANSPOSE while they split: TMA brings raw [32 pixels x w channels] pieces (w <= 32, hardware-swizzled so the
+// transposing reads are bank-conflict free), the consumers write hi/lo planes [channel row][32 pixels = 128 B] in
+// the K-major SWIZZLE_128B layout, and each warpgroup issues 4 K-steps x 3 products per 32-pixel stage into its
+// [64 x BN] half of ONE [128 x BN] accumulator that lives in registers for the CTA's whole pixel range.  The
+// planes are double-buffered: the split of stage i + 1 overlaps the MMAs of stage i.  Works for any channel
+// counts that are multiples of 4.  The bias gradient (column sums of G) is accumulated on the way.  One fp32
 // partial per CTA goes to the workspace; the fp32 path's fixed-order reduce kernel sums the partials
 // (deterministic) and scatters them into the Keras weight layout.
 // =============================================================================================
@@ -1064,18 +746,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
   constexpr int PLANE_G = BN * 128;
   constexpr int PLANES_BYTES = 2 * WG_PLANE_A + 2 * PLANE_G;      // Ahi, Alo, Ghi, Glo
-  constexpr uint32_t TMEM_COLS = BN <= 32 ? 32 : BN <= 64 ? 64 : 128;
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-  constexpr int GQ = BN / 4;                    // channel quads of G
-  constexpr int GI = (GQ + 3) / 4;              // G quads per transform thread
 
   extern __shared__ uint8_t smem_raw[];
   // offset arithmetic on the __shared__ array keeps the address space (LDS/STS instead of generic LD/ST)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  __shared__ __align__(8) uint64_t bars[2 * TC_MAX_STAGES + 5];
-  __shared__ uint32_t tmem_base_smem;
+  __shared__ __align__(8) uint64_t bars[2 * TC_MAX_STAGES];
   __shared__ WgPiece pieces[WG_MAX_PIECES];
-  __shared__ uint16_t items[64];            // work items of the transform: (piece << 8) | channel quad
+  __shared__ uint16_t items[64];            // work items of the split: (piece << 8) | channel quad
   __shared__ int n_pieces_s, n_items_s, raw_bytes_s;
   __shared__ float bias_part[64];
 
@@ -1084,9 +761,6 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
   const uint32_t bar0 = smem_u32(bars);
   auto bar_rfull = [&](int s) { return bar0 + 8u * s; };
   auto bar_rempty = [&](int s) { return bar0 + 8u * (TC_MAX_STAGES + s); };
-  auto bar_tready = [&](int b) { return bar0 + 8u * (2 * TC_MAX_STAGES + b); };
-  auto bar_tempty = [&](int b) { return bar0 + 8u * (2 * TC_MAX_STAGES + 2 + b); };
-  const uint32_t bar_accf = bar0 + 8u * (2 * TC_MAX_STAGES + 4);
   uint8_t* planes = smem;                                         // 2 x PLANES_BYTES
   uint8_t* raw = smem + 2 * PLANES_BYTES;                         // S x raw_stage_bytes
   const uint32_t planes_u32 = smem_u32(planes), raw_u32 = smem_u32(raw);
@@ -1134,32 +808,25 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
     }
     n_items_s = ni;
     raw_bytes_s = bytes;
-    for (int s = 0; s < S; ++s) { mbar_init(bar_rfull(s), 1); mbar_init(bar_rempty(s), 8); }      // one arrival per transform warp
-    for (int b = 0; b < 2; ++b) { mbar_init(bar_tready(b), 8); mbar_init(bar_tempty(b), 1); }
-    mbar_init(bar_accf, 1);
+    for (int s = 0; s < S; ++s) { mbar_init(bar_rfull(s), 1); mbar_init(bar_rempty(s), 8); }      // one arrival per consumer warp
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // transposed planes start as zero: rows beyond this tile's Kd / BN stay zero for the whole kernel
   for (int i = threadIdx.x; i < 2 * PLANES_BYTES / 16; i += TC_THREADS)
     reinterpret_cast<float4*>(planes)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_smem)),
-                 "r"(TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   const int n_pieces = n_pieces_s;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
   int my_tiles = 0;
   for (int t = blockIdx.x; t < p.total_ptiles; t += gridDim.x) ++my_tiles;
 
-  if (warp == 0) {
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < p.total_ptiles; t += gridDim.x) {
@@ -1191,32 +858,11 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      for (int i = 0; i < my_tiles; ++i) {
-        const int b = i & 1;
-        mbar_wait(bar_tready(b), (uint32_t)(i >> 1) & 1);
-        tc_fence_after();
-        const uint32_t ahi = planes_u32 + (uint32_t)b * PLANES_BYTES, alo = ahi + WG_PLANE_A;
-        const uint32_t ghi = alo + WG_PLANE_A, glo = ghi + PLANE_G;
-#pragma unroll
-        for (int ks = 0; ks < WG_PT / 8; ++ks) {
-          const uint64_t dah = umma_desc_kmajor<128>(ahi + ks * 32), dal = umma_desc_kmajor<128>(alo + ks * 32);
-          const uint64_t dgh = umma_desc_kmajor<128>(ghi + ks * 32), dgl = umma_desc_kmajor<128>(glo + ks * 32);
-          tc_mma_tf32(tmem_base, dal, dgh, IDESC, (i | ks) != 0);
-          tc_mma_tf32(tmem_base, dah, dgl, IDESC, 1);
-          tc_mma_tf32(tmem_base, dah, dgh, IDESC, 1);
-        }
-        tc_commit(bar_tempty(b));
-        if (i == my_tiles - 1) tc_commit(bar_accf);
-      }
-    }
   } else {
-    // ================= transpose + split: all eight remaining warps (2..9) =================
-    // ncu: with four warps this role ran one warp per scheduler at ~0.3 IPC (dependent LDS -> cvt -> STS
-    // chains) and set the stage time; eight warps and two independent items per thread hide that latency.
-    const int t = threadIdx.x - 64;               // 0..255 ; pixel = t % 32, item lane = t / 32
+    // ================= transpose + split, then wgmma: both consumer warpgroups (warps 4..11) =================
+    // every thread takes two independent items per stage (dependent LDS -> split -> STS chains need the parallelism)
+    const int wg = (warp >> 2) - 1;
+    const int t = threadIdx.x - 128;              // 0..255 ; pixel = t % 32, item lane = t / 32
     const int px = t & 31, ql = t >> 5;
     const int n_items = n_items_s;
     constexpr int MAXI = 6;                       // items per thread: 48 items / 8 lanes
@@ -1229,7 +875,6 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
     for (int it = 0; it < my_tiles; ++it) {
       const int b = it & 1;
       mbar_wait(bar_rfull(stage), phase);
-      mbar_wait(bar_tempty(b), ((uint32_t)(it >> 1) & 1) ^ 1);   // MMAs of two stages ago are done with planes b
       const uint8_t* rbase = raw + (size_t)stage * p.raw_stage_bytes;
       uint8_t* pl = planes + (size_t)b * PLANES_BYTES;
 #pragma unroll
@@ -1256,14 +901,30 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
           *reinterpret_cast<float*>(hi + lo_off + o) = tf32_round(vv[e] - h);
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> wgmma reads
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_tready(b));
-        mbar_arrive(bar_rempty(stage));
+      if (lane == 0) mbar_arrive(bar_rempty(stage));                  // raw stage consumed
+      // this warpgroup's MMAs of stage it - 1 are done; after the barrier, so are the other warpgroup's, and every
+      // warp has written planes b (planes b ^ 1 may be overwritten from the next stage on)
+      wgmma_wait_all();
+      acc_fence(acc);
+      named_bar_sync(1, 256);
+      const uint32_t ahi = planes_u32 + (uint32_t)b * PLANES_BYTES + (uint32_t)wg * (64 * 128), alo = ahi + WG_PLANE_A;
+      const uint32_t ghi = planes_u32 + (uint32_t)b * PLANES_BYTES + 2 * WG_PLANE_A, glo = ghi + PLANE_G;
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < WG_PT / 8; ++ks) {
+        const uint64_t dah = wgmma_desc<128>(ahi + ks * 32), dal = wgmma_desc<128>(alo + ks * 32);
+        const uint64_t dgh = wgmma_desc<128>(ghi + ks * 32), dgl = wgmma_desc<128>(glo + ks * 32);
+        wgmma_ss(acc, dal, dgh, 1);
+        wgmma_ss(acc, dah, dgl, 1);
+        wgmma_ss(acc, dah, dgh, 1);
       }
+      wgmma_commit();
       if (++stage == S) { stage = 0; phase ^= 1; }
     }
+    wgmma_wait_all();
+    acc_fence(acc);
     // bias partial: reduce the 32 pixel lanes of each warp in a fixed butterfly order
 #pragma unroll
     for (int i = 0; i < MAXI; ++i) {
@@ -1281,43 +942,23 @@ tc_wgrad_kernel(const __grid_constant__ WgMaps maps, const WgParams p) {
       }
     }
   }
-  // ---- all partials are ready: accumulator (after accf) and bias sums ----
+  // ---- all partials are ready: accumulators (registers of the consumers) and bias sums ----
   __syncthreads();
-  if (warp >= 6) {
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;            // accumulator row
-    const int k = k_lo + r;
-    if (my_tiles > 0) {
-      mbar_wait(bar_accf, 0);
-      tc_fence_after();
-    }
-    float* dst = p.ws + ((size_t)blockIdx.x * p.KD_pad + (k < k_hi ? k : 0)) * p.ld + ntile * BN;
-    const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16);
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      uint32_t v[16];
-      if (my_tiles > 0) {
-        tc_ld16(taddr + c0, v);
-      } else {
+  if (warp >= 4) {
+    const int wg = (warp >> 2) - 1, wq = warp & 3, g = lane >> 2, t4 = lane & 3;
 #pragma unroll
-        for (int e = 0; e < 16; ++e) v[e] = 0u;
-      }
+    for (int h = 0; h < 2; ++h) {
+      const int k = k_lo + 64 * wg + 16 * wq + g + 8 * h;         // accumulator row
       if (k < k_hi) {
+        float* dst = p.ws + ((size_t)blockIdx.x * p.KD_pad + k) * p.ld + ntile * BN + 2 * t4;
 #pragma unroll
-        for (int q4 = 0; q4 < 4; ++q4)
-          *reinterpret_cast<float4*>(dst + c0 + q4 * 4) =
-              make_float4(__uint_as_float(v[q4 * 4]), __uint_as_float(v[q4 * 4 + 1]), __uint_as_float(v[q4 * 4 + 2]),
-                          __uint_as_float(v[q4 * 4 + 3]));
+        for (int j = 0; j < BN / 8; ++j)
+          *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
       }
     }
+    const int r = threadIdx.x - 128;
     if (mtile == 0 && r < BN)
       p.ws[((size_t)blockIdx.x * p.KD_pad + p.bias_row) * p.ld + ntile * BN + r] = my_tiles > 0 ? bias_part[r] : 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
   }
 }
 
@@ -1380,7 +1021,7 @@ static WgPlan wg_plan(const GConvK& k) {
   }
   p.ntap_x = k.ax.nu; p.nseg = k.nseg; p.ctot = ctot;
   p.Kd = k.ay.nu * k.ax.nu * ctot;
-  if (p.Kd < 128) return pl;      // measured (also with 8 transform warps): below one full M tile the warp-stream fp32 kernel wins
+  if (p.Kd < 128) return pl;      // below one full M tile the warp-stream fp32 kernel takes the shape
   int coff = 0;
   for (int s = 0; s < k.nseg; ++s) { p.seg_C[s] = k.seg[s].C; p.seg_coff[s] = coff; coff += k.seg[s].C; }
   p.n_mtiles = (p.Kd + TC_BM - 1) / TC_BM;
@@ -1422,7 +1063,7 @@ static WgPlan wg_plan(const GConvK& k) {
   if (st < 2) return pl;
   p.raw_stages = st;
   pl.smem_bytes = planes + (size_t)st * p.raw_stage_bytes + 1024;
-  long long want = 148 / ((long long)p.n_mtiles * p.n_ntiles);
+  long long want = sm_count() / ((long long)p.n_mtiles * p.n_ntiles);
   if (want < 1) want = 1;
   if (want > tt / 4) want = tt / 4;
   if (want < 1) want = 1;
@@ -1529,16 +1170,16 @@ static int tc_launch_bn(const TcMaps& maps, const TcPlan& pl, cudaStream_t st) {
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !attr_set[pl.ts ? 1 : 0][dev]) {
-    cudaError_t e = pl.ts ? cudaFuncSetAttribute(tcs_gconv_kernel<BN, KBW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = pl.ts ? cudaFuncSetAttribute(tc_gconv_kernel<BN, KBW, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  227 * 1024 - 1024)
-                          : cudaFuncSetAttribute(tc_gconv_kernel<BN, KBW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                          : cudaFuncSetAttribute(tc_gconv_kernel<BN, KBW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  227 * 1024 - 1024);
     if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     if (dev >= 0 && dev < 64) attr_set[pl.ts ? 1 : 0][dev] = true;
   }
-  const int grid = pl.p.total_tiles < 148 ? pl.p.total_tiles : 148;
-  if (pl.ts) tcs_gconv_kernel<BN, KBW><<<grid, TCF_THREADS, pl.smem_bytes, st>>>(maps, pl.p);
-  else tc_gconv_kernel<BN, KBW><<<grid, TCF_THREADS, pl.smem_bytes, st>>>(maps, pl.p);
+  const int grid = pl.p.total_tiles < sm_count() ? pl.p.total_tiles : sm_count();
+  if (pl.ts) tc_gconv_kernel<BN, KBW, true><<<grid, TC_THREADS, pl.smem_bytes, st>>>(maps, pl.p);
+  else tc_gconv_kernel<BN, KBW, false><<<grid, TC_THREADS, pl.smem_bytes, st>>>(maps, pl.p);
   NLT_CUDA_LAUNCH_CHECK("tc_gconv_kernel");
   __atomic_add_fetch(&g_tc_launches, 1ull, __ATOMIC_RELAXED);
   return NLT_OK;
@@ -1554,7 +1195,7 @@ int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream
   float* blo = bhi + pl.pack_floats;
   const size_t total = pl.pack_floats;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   tc_pack_weights_kernel<<<blocks, 256, 0, st>>>(k, pl.kbw, pl.p.kb_total, pl.chunks_per_tap, pl.cout_pad, bhi, blo);
   NLT_CUDA_LAUNCH_CHECK("tc_pack_weights_kernel");
   return NLT_OK;

@@ -2,11 +2,11 @@
 // convs of the level-1 blocks (nlt/networks/convnet.py:50-59, 67-76 at depth0 = 16: 4 -> 4 and 8 -> 8 channels at
 // 1024^2 / 512^2, 16 -> 16 at 512^2).  They move 30-130 bytes per pixel for 64-1024 FMAs: pure streams, for which the
 // general small-stencil kernel (nlt_small.cu: any tap set, any pixel map, runtime segment lists, 64-bit pixel decode per
-// thread) spends several hundred instructions of bookkeeping per pixel and reaches 1.0-1.5 TB/s.
+// thread) spends several hundred instructions of bookkeeping per pixel.
 //
 // Here a CTA owns a run of consecutive pixels of ONE lattice row: the image / row decode happens once per CTA, a
 // thread's addresses are `row base + x * C`, tap rows that fall outside the image are skipped for the whole CTA, all
-// channel loops are compile-time, weights come from constant memory (uniform datapath) into FFMA2.
+// channel loops are compile-time, weights come from constant memory as FMA operands.
 #include "nlt_common.cuh"
 
 namespace nlt {
@@ -88,7 +88,7 @@ tiny_stencil_kernel(const TinyParams p) {
             const float2 xx = make_float2(xs[e], xs[e]);
             const float2* w = tiny_cw + (kbase + 4 * q + e) * (COUT / 2);
 #pragma unroll
-            for (int m = 0; m < COUT / 2; ++m) acc[m] = __ffma2_rn(xx, w[m], acc[m]);
+            for (int m = 0; m < COUT / 2; ++m) acc[m] = ffma2(xx, w[m], acc[m]);
           }
         }
       }

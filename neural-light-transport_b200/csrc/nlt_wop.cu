@@ -6,7 +6,7 @@
 //
 // Their [K_d x N] products are tiny (64 ... 10240 numbers) and the pixel streams long (0.5-8 M pixels), so the work
 // is cut into OUTER-PRODUCT UNITS: per lattice pixel a unit multiplies one float4 "A" (4 channels of one operand)
-// with 16 consecutive floats "B" of the other operand into a 4 x 16 register tile (32 FFMA2 for 5 LDG.128).  A warp
+// with 16 consecutive floats "B" of the other operand into a 4 x 16 register tile (64 FMAs for 5 LDG.128).  A warp
 // owns one unit kind for the whole launch (its accumulators never leave registers): lanes = (pixel slot, channel quad
 // of A) with the quad fastest, so that A loads are one contiguous 512-byte run and B loads broadcast inside a pixel.
 // Warps stream over row tiles on their own -- no shared memory, no barriers -- and write one fp32 partial per CTA in
@@ -109,8 +109,8 @@ wop_wgrad_kernel(const __grid_constant__ WopParams p, float* __restrict__ ws) {
         const float2 aa = make_float2(as[i], as[i]);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          acc[i][2 * j] = __ffma2_rn(aa, make_float2(bv[j].x, bv[j].y), acc[i][2 * j]);
-          acc[i][2 * j + 1] = __ffma2_rn(aa, make_float2(bv[j].z, bv[j].w), acc[i][2 * j + 1]);
+          acc[i][2 * j] = ffma2(aa, make_float2(bv[j].x, bv[j].y), acc[i][2 * j]);
+          acc[i][2 * j + 1] = ffma2(aa, make_float2(bv[j].z, bv[j].w), acc[i][2 * j + 1]);
         }
       }
     }
@@ -139,9 +139,9 @@ wop_wgrad_kernel(const __grid_constant__ WopParams p, float* __restrict__ ws) {
     }
 }
 
-// option "wop" / NLT_WOP: 0 off; 1 (default) the 4 -> 4 and 8 -> 8 stencils, where it wins (q12.1: 0.262 -> 0.206 ms,
-// q11.1: 0.167 -> 0.156 ms, profiles/r2_q_*); 2 also the 16 -> 16 stencils and the up-convs, which are correct but
-// 1.1-2x SLOWER than the staged-patch / tcgen05 kernels (16 warps/SM at 128 registers cannot hide the load latency)
+// option "wop" / NLT_WOP: 0 off; 1 (default) the 4 -> 4 and 8 -> 8 stencils; 2 also the 16 -> 16 stencils and the
+// up-convs, which are correct but slower than the staged-patch / wgmma kernels (16 warps/SM at 128 registers cannot
+// hide the load latency)
 int g_opt_wop = -1;
 static int wop_level() {
   if (g_opt_wop < 0) { const char* e = getenv("NLT_WOP"); g_opt_wop = e ? atoi(e) : 1; }
@@ -277,7 +277,7 @@ static WopPlan wop_plan(const GConvK& k, const float* G) {
   p.ntiles = (uint32_t)ntiles;
   // 128 registers per thread: 16 resident warps per SM
   const unsigned per_sm = (unsigned)(16 / nt > 0 ? 16 / nt : 1);
-  const unsigned cap = 148u * per_sm;
+  const unsigned cap = (unsigned)sm_count() * per_sm;
   pl.grid = p.ntiles < cap ? (unsigned)p.ntiles : cap;
   pl.ok = true;
   return pl;
@@ -406,7 +406,7 @@ static bool wopn_plan(const GConvK& k, const float* G, WopnParams* p, unsigned* 
   if (p->w_seg[0] != 0) return false;
   p->nwarp = nw; p->N = k.Cout; p->ld = (k.Cout + 3) / 4 * 4;
   p->kd_pad = (GS + 1) * 4; p->bias_row = GS * 4; p->M = k.M;
-  *grid = 148u * (unsigned)(nw <= 4 ? 8 : (nw <= 8 ? 5 : 4));
+  *grid = (unsigned)sm_count() * (unsigned)(nw <= 4 ? 8 : (nw <= 8 ? 5 : 4));
   *GS_out = GS;
   return true;
 }

@@ -185,8 +185,7 @@ class use_workspaces:
         return False
 _SIDE = {}                   # (device index, i) -> side stream
 # weight-gradient streams (NLT_SIDE_STREAMS, default 2): consecutive layers' weight gradients go round-robin to
-# different streams, so that the latency-bound launches of the deep levels overlap each other too (cfg4 step 14.83 ->
-# 14.72 ms with 2, no further gain with 3 or 4: profiles/r2_r_*)
+# different streams, so that the latency-bound launches of the deep levels overlap each other too
 N_SIDE_STREAMS = max(1, int(os.environ.get('NLT_SIDE_STREAMS', '2')))
 _side_rr = [0]
 
@@ -218,10 +217,9 @@ FWD_TAP = None
 
 
 # NLT_PACK_AHEAD (default 0): weight planes of the tensor-core layers are packed on a stream that hangs off the START
-# of the step (weights are final there) instead of in front of each layer's kernel on the main stream.  Measured
-# (profiles/r2_s_*, r2_t_*): inside the captured CUDA graph the ~60 pack nodes do not start earlier than before (14.83
-# vs 14.74 ms per step), and eager launches pay the extra stream switches on the host -- so the switch stays off; the
-# C-ABI entry points and the scheduling-invariance test remain.
+# of the step (weights are final there) instead of in front of each layer's kernel on the main stream.  Inside the
+# captured CUDA graph the pack nodes do not start earlier than before, and eager launches pay the extra stream switches
+# on the host -- so the switch stays off; the C-ABI entry points and the scheduling-invariance test remain.
 PACK_AHEAD = os.environ.get('NLT_PACK_AHEAD', '0') == '1'
 _PACK = {}                   # device index -> pack stream
 _STEP_ROOT = {}              # device index -> [event recorded on the main stream at step begin, forked?]

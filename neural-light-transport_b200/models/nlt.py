@@ -1,10 +1,10 @@
-"""NLT model on the B200 hot path -- mirror of nlt/models/nlt.py:38-205.
+"""NLT model on the CUDA hot path -- mirror of nlt/models/nlt.py:38-205.
 
 Same surface as the reference: `Model(config)`, `register_trainable()`,
 `model(batch, mode=)` == `model.call(batch, mode, obs_override=None)` ->
 `(pred_camspc, gt_camspc, loss_kwargs, to_vis)`, `_call(query_x, obs_xs,
 obs_weights, obs_override)`, `compute_loss(pred, gt, **kw)`, `.net` dict,
-`.trainable_variables`.  The arithmetic is executed by hand-written sm_100a
+`.trainable_variables`.  The arithmetic is executed by hand-written sm_90a
 kernels (include/nlt_b200.h) over a virtual channel concat: no tf.concat,
 no `nn_rgb - nn_base`, no K-stack and no standalone bias/activation pass is
 ever materialised.  Gradients are produced by `model.backward()` (the

@@ -51,6 +51,7 @@ _SIGS = {
     'nlt_set_option': (C.c_int, [C.c_char_p, C.c_int]),
     'nlt_launch_count': (C.c_uint64, []),
     'nlt_tc_launch_count': (C.c_uint64, []),
+    'nlt_kernel_launch_count': (C.c_uint64, [C.c_char_p]),
     'nlt_gconv_fwd': (C.c_int, [C.POINTER(GConvDesc), C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_int,
                                 C.c_void_p, C.c_void_p]),
     'nlt_gconv_fwd_fused_supported': (C.c_int, [C.POINTER(GConvDesc), C.POINTER(PwTerm), C.c_void_p, C.c_void_p]),
@@ -88,7 +89,6 @@ _SIGS = {
     'nlt_instnorm_workspace_bytes': (C.c_int64, [C.c_int32] * 3),
     'nlt_instnorm_fwd': (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_int, C.c_float] + [C.c_void_p] * 5),
     'nlt_instnorm_bwd': (C.c_int, [C.c_void_p] * 5 + [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 2),
-    'nlt_debug_tcts_probe': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     'nlt_u8_to_f32': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'nlt_ksum_acc': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     'nlt_scale': (C.c_int, [C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
@@ -141,11 +141,16 @@ def launch_count():
     return int(lib().nlt_launch_count())
 
 
+def kernel_launch_count(name):
+    """Launches of the kernel the library reports as `name` so far."""
+    return int(lib().nlt_kernel_launch_count(name.encode()))
+
+
 def tc_launch_count():
-    """tcgen05 tensor-core kernel launches so far."""
+    """wgmma tensor-core kernel launches so far."""
     return int(lib().nlt_tc_launch_count())
 
 
 def set_option(name, value):
-    """'tc' / 'tc_wgrad': 1 = tcgen05 3xTF32 kernels where eligible (default), 0 = fp32-FMA kernels only."""
+    """'tc' / 'tc_wgrad': 1 = wgmma 3xTF32 kernels where eligible (default), 0 = fp32-FMA kernels only."""
     check(lib().nlt_set_option(name.encode(), int(value)))

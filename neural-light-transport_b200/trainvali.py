@@ -57,7 +57,7 @@ def get_strategy(device='gpu'):
     if device == 'cpu':
         # the reference offers OneDeviceStrategy('/cpu:0'); this hot path has
         # no CPU implementation by design
-        raise NotImplementedError('device=cpu: the B200 hot path has no CPU fallback')
+        raise NotImplementedError('device=cpu: the CUDA hot path has no CPU fallback')
     raise NotImplementedError(device)
 
 
@@ -261,6 +261,10 @@ class GraphedTrainStep:
                 # NCCL creates its communicator at the first collective, which cannot happen inside a capture
                 self.strategy.all_reduce_sum_(torch.zeros(1, device=dev))
             torch.cuda.synchronize()
+            # the warm-up ran on a side stream: its freed activation blocks stay cached for that stream, where the
+            # graph's private pool cannot reuse them.  Returning them first keeps the step's peak at one set of
+            # activations (cfg4 at batch 32 does not fit in 80 GB otherwise)
+            torch.cuda.empty_cache()
             it0 = self.optimizer.iterations
             self.optimizer._state(self.model.flat_params)
             for full in ([True, False] if self.graph_collectives else [False]):

@@ -12,8 +12,8 @@ this restatement is pinned only by (i) hand-computed known-answer vectors,
 (ii) an independent direct-loop numpy restatement (oracle/np_ref.py), and
 (iii) the one docstring example the reference carries (util/net.py:23).
 
-Every function cites the reference file:line it follows (paths relative to
-/root/reference).  External-op semantics (TF 2.2 Conv2D/Conv2DTranspose 'same',
+Every function cites the reference file:line it follows (paths relative to a
+checkout of google/neural-light-transport).  External-op semantics (TF 2.2 Conv2D/Conv2DTranspose 'same',
 tfa.image.resampler 0.10, tf.image.resize, Keras Adam(amsgrad)) are restated
 from their published behaviour; see SURVEY.md section 8c.
 """

@@ -1,5 +1,5 @@
-"""Builds tests/golden/barron_reference_fixtures.npz from the reference's OWN test fixtures (run in the container
-that has /root/reference; the GPU box only sees the committed npz):
+"""Builds tests/golden/barron_reference_fixtures.npz from the reference's OWN test fixtures (argument: a checkout
+of google/neural-light-transport; the tests only read the committed npz):
 
   * third_party/robust_loss/data/wavelet_golden.mat -- an 83 x 71 RGB image and its 5-level CDF 9/7 pyramid made
     by an independent implementation (see wavelet_test.py:146-172); stored here as float64 arrays
@@ -7,11 +7,12 @@ that has /root/reference; the GPU box only sees the committed npz):
   * third_party/robust_loss/data/partition_spline.npz -- only `x_scale` and the two knots around alpha = 1.
 """
 import os
+import sys
 
 import numpy as np
 import scipy.io
 
-REF = '/root/reference/third_party/robust_loss/data'
+REF = os.path.join(sys.argv[1] if len(sys.argv) > 1 else '.', 'third_party', 'robust_loss', 'data')
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'barron_reference_fixtures.npz')
 
 

@@ -1,10 +1,10 @@
 """Generates the committed fixtures of tests/golden/.
 
-  python tests/golden/make_golden.py            # rewrites the .npz files
+  python tests/golden/make_golden.py REFERENCE_CHECKOUT   # rewrites the .npz files
 
 * gen_feat_n_reference.npz -- outputs of the REFERENCE's own
   nlt/util/net.py:gen_feat_n (the only module on the path importable without
-  TensorFlow), imported from /root/reference in this container.
+  TensorFlow), imported from a checkout of google/neural-light-transport.
 * model_h64.npz -- fp64 run of oracle/nlt_oracle.py (the restated reference) on
   a seeded 64x64 dragon_specular-shaped problem: forward, loss, gradients.
   NOTE: this pins the oracle against regressions; the reference itself has no
@@ -56,7 +56,7 @@ def compute(dtype=torch.float64):
 
 
 def main():
-    spec = importlib.util.spec_from_file_location('refnet', '/root/reference/nlt/util/net.py')
+    spec = importlib.util.spec_from_file_location('refnet', os.path.join(sys.argv[1], 'nlt', 'util', 'net.py'))
     ref = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(ref)
     gf = {}

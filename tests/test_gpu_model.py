@@ -70,7 +70,7 @@ def run_pair(over, B=2, seed=1234, c_extra=0, im=None):
 @pytest.fixture(params=['fp32', 'tc'])
 def path(request):
     """Runs a test on both execution paths of the library: 'fp32' = fp32-FMA kernels only (strict parity
-    bar), 'tc' = tcgen05 3xTF32 kernels wherever a shape is eligible (the default, performance path)."""
+    bar), 'tc' = wgmma 3xTF32 kernels wherever a shape is eligible (the default, performance path)."""
     import nlt_native as nat
     nat.set_option('tc', 1 if request.param == 'tc' else 0)
     yield request.param

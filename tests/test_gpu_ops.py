@@ -61,7 +61,7 @@ GEOMS = [
     ('deconv', 2, 2, 128, 256, [8, 32], 4),
     ('conv', 2, 1, 256, 256, [16], 16),
     ('deconv', 2, 2, 64, 64, [32, 64], 32),
-    # tensor-core (tcgen05, 3xTF32) eligible shapes: every source C % 32 == 0, Cout % 16 == 0, tileable lattice
+    # tensor-core (wgmma, 3xTF32) eligible shapes: every source C % 32 == 0, Cout % 16 == 0, tileable lattice
     ('conv', 2, 2, 32, 32, [32, 32], 64),       # patch view (5-D TMA), lattice 16x16 -> tile 8x16
     ('conv', 2, 1, 16, 16, [64], 64),           # stride-1 taps, SAME pad by TMA OOB fill
     ('conv', 3, 1, 16, 16, [32], 32),           # negative start coordinates
@@ -89,7 +89,7 @@ GEOMS = [
     ('conv', 2, 2, 32, 128, [32, 32], 64),      # ... lattice rows narrower than a tile: two rows per tile
     ('conv', 2, 2, 32, 128, [16], 16),          # ... four lattice rows per tile, 16-channel source
     ('conv', 2, 2, 32, 128, [32], 32),          # K = 32 -> 4 x 32
-    # staged-patch FFMA2 weight gradient of the 2x2 convs (pws_wgrad_kernel): all four lane layouts, both strides,
+    # staged-patch weight gradient of the 2x2 convs (pws_wgrad_kernel): all four lane layouts, both strides,
     # SAME padding at the right / bottom edge
     ('conv', 2, 2, 16, 256, [16, 16], 16),      # K = 128, N = 16
     ('conv', 2, 1, 8, 128, [16], 32),           # K = 64, N = 32, stride 1
@@ -173,7 +173,7 @@ WOP_ALL_SHAPES = [g for g in GEOMS if g[4] >= 32 and (
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', WOP_ALL_SHAPES)
 def test_outer_product_wgrad_all_shapes(kind, k, s, H, W, segc, cout):
     """nlt_wop.cu also serves the up-convs and the 16 -> 16 stencils (option wop = 2; off by default because the
-    staged-patch / tcgen05 kernels are faster there): same oracle check as every other route."""
+    staged-patch / wgmma kernels are faster there): same oracle check as every other route."""
     import nlt_native as nat
     nat.set_option('wop', 2)
     try:
@@ -189,15 +189,38 @@ NS2_SHAPES = [g for g in GEOMS if g[6] in (16, 32) and g[4] >= 128 and (
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', NS2_SHAPES)
 def test_two_threads_per_pixel_forward_kernels(kind, k, s, H, W, segc, cout):
     """The pointwise / staged-patch forward kernels also exist with two threads per pixel (options pwx_ns / pf_ns = 2,
-    off by default: not faster, profiles/r2_u_*): same oracle check."""
+    off by default): same oracle check."""
     import nlt_native as nat
     nat.set_option('pwx_ns', 2)
     nat.set_option('pf_ns', 2)
+    nat.set_option('pf', 1)
     try:
         test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
     finally:
         nat.set_option('pwx_ns', 1)
         nat.set_option('pf_ns', 1)
+        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
+
+
+@pytest.mark.parametrize('kind,k,s,H,W,segc,cout', [('conv', 2, 2, 4, 512, [16], 32), ('conv', 2, 2, 4, 256, [32], 16),
+                                                    ('conv', 2, 2, 6, 256, [16, 16], 16), ('conv', 2, 2, 16, 256, [32], 64),
+                                                    ('conv', 2, 2, 32, 128, [32, 32], 64)])
+def test_staged_patch_forward_and_pwd2s_first_routes(kind, k, s, H, W, segc, cout):
+    """Options pf (staged-patch forward of the 2x2/s2 convs) and pwd2s_first (depth-to-space input gradient ahead of
+    the tensor path for 64-channel gradients), both off by default: same oracle check on the routes they select, and
+    the kernel of the route must have run (K = 64 / 128 forwards into 16 / 32 channels: pf_fwd_kernel; input gradients
+    into 16- / 32-channel sources: pwd2s_kernel)."""
+    import nlt_native as nat
+    kernel = 'pf_fwd_kernel' if H in (4, 6) else 'pwd2s_kernel'
+    nat.set_option('pf', 1)
+    nat.set_option('pwd2s_first', 1)
+    try:
+        n0 = nat.kernel_launch_count(kernel)
+        test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
+        assert nat.kernel_launch_count(kernel) > n0, kernel + ' did not run'
+    finally:
+        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
+        nat.set_option('pwd2s_first', int(os.environ.get('NLT_PWD2S_FIRST', '0')))
 
 
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', [('conv', 2, 1, 5, 128, [16], 16), ('deconv', 2, 1, 5, 256, [16], 16),
@@ -207,11 +230,15 @@ def test_staged_patch_kernel_on_stride1_stencils(kind, k, s, H, W, segc, cout):
     SAME padding on either side (conv / deconv flavour)."""
     import nlt_native as nat
     nat.set_option('pf_s1', 1)
+    nat.set_option('pf', 1)
     try:
         for act in ('leakyrelu', None):
+            n0 = nat.kernel_launch_count('pf_fwd_kernel')
             test_gconv_forward_backward(kind, k, s, H, W, segc, cout, act)
+            assert nat.kernel_launch_count('pf_fwd_kernel') > n0, 'pf_fwd_kernel did not run'
     finally:
         nat.set_option('pf_s1', int(os.environ.get('NLT_PF_S1', '0')))
+        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
 
 
 TC_SHAPES = [g for g in GEOMS if all(c % 16 == 0 for c in g[5]) and g[6] % 16 == 0 and g[3] * g[4] >= 256]
@@ -220,35 +247,41 @@ TC_SHAPES = [g for g in GEOMS if all(c % 16 == 0 for c in g[5]) and g[6] % 16 ==
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', [g for g in GEOMS if all(c % 16 == 0 for c in g[5]) and g[6] % 16 == 0
                                                     and g[3] * g[4] >= 256][:14])
 def test_tensor_core_raw_hi_operand(kind, k, s, H, W, segc, cout):
-    """Option tc_rawhi: the activation tile as TMA delivered it is the hi operand (the tensor core ignores the low 13
-    bits), only lo = x - trunc(x) is written by the transform warps.  Same oracle check, same tolerance (a core that
-    ROUNDED its operands would be 1e-3 off here)."""
+    """Option tc_rawhi: the hi operand is the activation truncated to TF32 (lo = x - trunc(x), exact before its own
+    rounding) or, with 0, rounded to TF32.  Same oracle check, same tolerance for both splits; option tc = 2 puts every
+    shape on the wgmma kernel, and its launch counter must move."""
     import nlt_native as nat
+    nat.set_option('tc', 2)
     try:
-        for v in (1, 0):         # default form, and the one that writes a rounded hi plane
+        for v in (1, 0):         # default form, and the one that rounds hi
             nat.set_option('tc_rawhi', v)
+            n0 = nat.tc_launch_count()
             test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
+            assert nat.tc_launch_count() > n0, 'tensor-core kernel did not run'
     finally:
         nat.set_option('tc_rawhi', int(os.environ.get('NLT_TC_RAWHI', '1')))
+        nat.set_option('tc', 1)
 
 
 @pytest.fixture(params=['ss', 'ts'])
 def tc_form(request):
-    """Both forms of the tcgen05 forward / input-gradient kernel: 'ss' = operands in shared memory after an smem -> smem
-    split (round 1), 'ts' = the activation operand converted on its way into tensor memory (round 2)."""
+    """Both forms of the wgmma forward / input-gradient kernel: 'ss' = hi / lo activation planes written to shared
+    memory (both operands from shared memory), 'ts' = the activation operand split in registers (wgmma RS form)."""
     import nlt_native as nat
     nat.set_option('tcs', 1 if request.param == 'ts' else 0)
     yield request.param
     nat.set_option('tcs', int(os.environ.get('NLT_TCS', '%d' % TCS_DEFAULT)))
 
 
-TCS_DEFAULT = 0
+TCS_DEFAULT = 1
 
 
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', TC_SHAPES)
 def test_tensor_core_vs_fp32_kernels(kind, k, s, H, W, segc, cout, tc_form):
-    """A/B on identical inputs: tcgen05 3xTF32 kernels (forward, input gradients with beta + mask, weight /
-    bias gradients) against the fp32-FMA kernels of the same library: relative Frobenius error <= 5e-6."""
+    """A/B on identical inputs: wgmma 3xTF32 kernels (forward, input gradients with beta + mask, weight /
+    bias gradients) against the fp32-FMA kernels of the same library: relative Frobenius error <= 5e-6.  The tensor-core
+    arm runs with option tc = 2, so that every shape the wgmma kernel can run takes it, whatever the size heuristics
+    would pick in production."""
     engine, nat = _mods()
     dev = torch.device('cuda')
     torch.manual_seed(3)
@@ -257,7 +290,7 @@ def test_tensor_core_vs_fp32_kernels(kind, k, s, H, W, segc, cout, tc_form):
     dzs = None
     res = {}
     for mode in ('tc', 'fp32'):
-        nat.set_option('tc', 1 if mode == 'tc' else 0)
+        nat.set_option('tc', 2 if mode == 'tc' else 0)
         L = engine.ConvLayer(kind, k, s, cout, 'leakyrelu')
         L.build(sum(segc), dev, torch.Generator().manual_seed(1))
         L.bias.copy_(torch.linspace(-0.1, 0.1, cout, device=dev))
@@ -273,8 +306,7 @@ def test_tensor_core_vs_fp32_kernels(kind, k, s, H, W, segc, cout, tc_form):
                          tc=nat.tc_launch_count() - t0)
     nat.set_option('tc', 1)
     assert res['fp32']['tc'] == 0
-    if res['tc']['tc'] == 0:
-        pytest.skip('shape is routed to the fp32 kernels by the measured dispatch heuristics')
+    assert res['tc']['tc'] > 0
     rel = lambda a, b: float((a.double() - b.double()).norm() / b.double().norm())
     assert rel(res['tc']['y'], res['fp32']['y']) <= 1e-5      # 3xTF32: ~1e-6 per product, grows ~sqrt(K)
     # weight / bias gradients sum over every pixel: both paths carry fp32 accumulation error of their own
@@ -481,7 +513,7 @@ def test_wide_stencil_8_outputs_and_virtual_concats(kind, k, s, H, W, segc, cout
 
 
 def test_tensor_core_path_is_taken_and_matches_fp32_path():
-    """Eligible shapes must run on the tcgen05 kernel (launch counter moves) and agree with the
+    """Eligible shapes must run on the wgmma kernel (launch counter moves) and agree with the
     fp32-FMA kernel of the same library to 3xTF32 accuracy (<= 4e-6 relative to the output scale)."""
     import ctypes as C
     engine, nat = _mods()

@@ -84,8 +84,8 @@ def main():
                'graph_vs_single_rel_displacement': g_rel, 'eager_vs_single_max': e_max,
                'eager_vs_single_rel_displacement': e_rel, 'loss_rel_graph': l_err, 'loss_rel_eager': le_err, 'ok': ok}
         print(json.dumps(out))
-    # leave without tearing the communicator down: on 2 GPUs (round 2, call X) the result above was printed and the
-    # processes then sat in destroy_process_group() until the 600 s timeout -- rank 1 reaches it minutes before rank 0
+    # leave without tearing the communicator down: on 2 GPUs the result above was printed and the processes then sat
+    # in destroy_process_group() until the job timed out -- rank 1 reaches it minutes before rank 0
     # (which still computes the single-replica reference) while CUDA graphs holding NCCL kernels are alive
     if world > 1:
         torch.distributed.barrier()
