@@ -28,6 +28,26 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
+// ---- 3xTF32 operand split (the wgmma kernels of nlt_tc.cu, the mma.sync kernels of nlt_pwx.cu) ----------------
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
+// Round-to-nearest TF32 in two integer instructions (cvt.rna.tf32 expands to several instructions with its inf/nan
+// handling).  Adding half an ulp to the bit pattern and clearing the low 13 mantissa bits rounds the magnitude to
+// nearest (ties away), carries into the exponent correctly, and is only wrong for inf/nan, which the split does not
+// need to preserve.
+__device__ __forceinline__ float tf32_round(float x) {
+  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+}
+// 3xTF32 split of one activation: hi = x truncated (rawhi) or rounded to TF32; lo = x - hi (exact), rounded to TF32
+__device__ __forceinline__ void tf32_split(float x, int rawhi, uint32_t& hi, uint32_t& lo) {
+  const float h = rawhi ? __uint_as_float(__float_as_uint(x) & 0xFFFFE000u) : tf32_round(x);
+  hi = __float_as_uint(h);
+  lo = __float_as_uint(tf32_round(x - h));
+}
+
 // ---- division by an invariant (Granlund-Montgomery), n < 2^31 ----------------
 struct FastDiv {
   uint32_t d, m, l;
@@ -205,6 +225,11 @@ bool pwd2s_applicable(const GConvK& k, const float* bias, int act, const float* 
                       const PwExtra* ex);
 int launch_pwd2s(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
                  const PwExtra* ex);
+// the same op on the tensor cores (mma.sync 3xTF32), for every shape pwd2s_applicable accepts; option "pwmma"
+extern int g_opt_pwmma;
+bool pwmma_enabled();
+int launch_pwd2s_mma(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
+                     const PwExtra* ex);
 
 // weight gradient of the 2x2 convs of the 16- / 32-channel levels (staged input patch, nlt_pwx.cu)
 bool pws_wgrad_applicable(const GConvK& k, const float* G);

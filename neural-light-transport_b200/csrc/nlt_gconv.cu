@@ -730,6 +730,13 @@ static bool tc_wgrad_enabled() {
   return tc_enabled() && g_opt_tc_wgrad == 1;
 }
 
+// depth-to-space input gradient: the tensor-core form unless tc = 0 or pwmma = 0 (then the fp32 FMA kernel)
+static int launch_pwd2s_route(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
+                              const PwExtra* ex) {
+  if (tc_enabled() && pwmma_enabled()) return launch_pwd2s_mma(k, beta, mask_y, mask_act, out, st, ex);
+  return launch_pwd2s(k, beta, mask_y, mask_act, out, st, ex);
+}
+
 int nlt_set_option(const char* name, int value) {
   NLT_CHECK_ARG(name != nullptr, "null option name");
   if (strcmp(name, "tc") == 0) { g_opt_tc = value ? 1 : 0; nlt::g_tc_force = value == 2; return NLT_OK; }
@@ -737,6 +744,7 @@ int nlt_set_option(const char* name, int value) {
   if (strcmp(name, "wgrad_rows") == 0) { nlt::g_opt_wgrad_rows = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "tcs") == 0) { nlt::g_opt_tcs = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "pwx") == 0) { nlt::g_opt_pwx = value ? 1 : 0; return NLT_OK; }
+  if (strcmp(name, "pwmma") == 0) { nlt::g_opt_pwmma = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "tc_rawhi") == 0) { nlt::g_opt_tc_rawhi = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "pwd2s_first") == 0) { g_opt_pwd2s_first = value ? 1 : 0; return NLT_OK; }
   if (strcmp(name, "pf_s1") == 0) { nlt::g_opt_pf_s1 = value ? 1 : 0; return NLT_OK; }
@@ -845,7 +853,7 @@ static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, f
     const GConvK& k = ph[i];
     if (k.M == 0) continue;
     if (pwx_fwd_applicable(k, beta, mask_y, out)) rc = launch_pwx_fwd(k, bias, act, out, st);
-    else if (pwd2s_applicable(k, bias, act, out, mask_y, nullptr)) rc = launch_pwd2s(k, beta, mask_y, mask_act, out, st, nullptr);
+    else if (pwd2s_applicable(k, bias, act, out, mask_y, nullptr)) rc = launch_pwd2s_route(k, beta, mask_y, mask_act, out, st, nullptr);
     else if (pw_conv_applicable(k)) rc = launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, st);
     else if (tiny_stencil_applicable(k, out, mask_y)) rc = launch_tiny_stencil(k, bias, act, beta, mask_y, mask_act, out, st);
     // option "dconv_wide_first" (default on): prefer the wide stencil kernel over the quad-per-thread one where both apply
@@ -895,7 +903,7 @@ int nlt_gconv_fwd_fused(const nlt_gconv_desc* d, const nlt_pw_term* term, const 
   NLT_CHECK_ARG(act >= 0 && act <= 3 && mask_act >= 0 && mask_act <= 3, "bad activation code");
   NLT_CHECK_ARG(beta == 0.f || beta == 1.f, "beta must be 0 or 1");
   if (k.M > 0 && pwd2s_applicable(k, bias, act, out, mask_y, &ex))
-    return launch_pwd2s(k, beta, mask_y, mask_act, out, (cudaStream_t)stream, &ex);
+    return launch_pwd2s_route(k, beta, mask_y, mask_act, out, (cudaStream_t)stream, &ex);
   if (k.M == 0 || !pw_extra_applicable(k, ex, out, mask_y))
     return set_err(NLT_ERR_UNSUPPORTED, "fused pointwise term: shape not served by the pointwise kernel");
   return launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, (cudaStream_t)stream, &ex);

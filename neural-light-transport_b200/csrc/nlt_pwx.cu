@@ -970,6 +970,10 @@ struct PwdParams {
   int ex_K;
   const float* ex_w;
   long long ex_wk, ex_wn;
+  // the layer's weights W[tap][k][c] = w[tap * wt + k * wc + c * wn] and the activation split (pwd2s_mma_kernel only)
+  const float* w;
+  long long wt, wc, wn;
+  int rawhi;
 };
 
 __global__ void pwd_pack_w_kernel(const GConvK g, int K, int CS) {
@@ -983,6 +987,72 @@ __global__ void pwd_pack_w_kernel(const GConvK g, int K, int CS) {
   }
 }
 
+// weights of the fused pointwise term, [PW_EX_KMAX][CS] (zero beyond ex_K)
+template <int CS>
+__device__ __forceinline__ void pwd_load_exw(const PwdParams& p, float* exw) {
+  for (int i = threadIdx.x; i < PW_EX_KMAX * CS; i += PWD_THREADS)
+    exw[i] = (p.ex_x != nullptr && i < p.ex_K * CS)
+                 ? __ldg(p.ex_w + (long long)(i / CS) * p.ex_wk + (long long)(i % CS) * p.ex_wn) : 0.f;
+}
+
+// ---- coalesced output runs of one staged tile (so: [TP][SROW], column n' = tap * CS + c): per lattice row of the
+// tile, rows 2*row and 2*row + 1 of the output, 2*wtile pixels of CS channels each.  TP*CS float4 per tile, in
+// batches of 4 per thread: every read-modify-write operand of a batch is requested before the first one is used ----
+template <int TP, int CS, int SROW>
+__device__ __forceinline__ void pwd_store_tile(const PwdParams& p, const float* so, const float* exw, uint32_t row0,
+                                               uint32_t x0) {
+  constexpr int C4 = CS / 4;
+  constexpr int PER_THREAD = TP * CS / PWD_THREADS;
+  const int tid = threadIdx.x;
+  const int Wout = 2 * p.Win;
+  const int wtile = p.Win < TP ? p.Win : TP;                       // lattice pixels per row inside a tile
+#pragma unroll 1
+  for (int b4 = 0; b4 < PER_THREAD / 4; ++b4) {
+    float4 v[4], old[4], ym[4];
+    float xe[4][PW_EX_KMAX];
+    uint32_t o4[4];                                                // float4 index into out (pwd2s_applicable: < 2^32)
+    int jq[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int f = tid + (b4 * 4 + u) * PWD_THREADS;              // float4 index inside the tile's outputs
+      const int j = f % C4;                                        // C4, 2 * wtile: powers of two
+      int r = f / C4;
+      const int ox = r & (2 * wtile - 1);
+      r >>= p.lw2;
+      const int dy = r & 1, lr = r >> 1;                           // output row parity, lattice row inside the tile
+      const int px = lr * wtile + (ox >> 1), dx = ox & 1;
+      jq[u] = j;
+      o4[u] = ((2 * (row0 + lr) + dy) * (uint32_t)Wout + 2 * x0 + ox) * C4 + j;
+      if (p.beta != 0.f) old[u] = reinterpret_cast<const float4*>(p.out)[o4[u]];
+      if (p.mask_y != nullptr) ym[u] = __ldg(reinterpret_cast<const float4*>(p.mask_y) + o4[u]);
+      if (p.ex_x != nullptr) {
+#pragma unroll
+        for (int k = 0; k < PW_EX_KMAX; ++k) xe[u][k] = k < p.ex_K ? __ldg(p.ex_x + (size_t)(o4[u] / C4) * p.ex_K + k) : 0.f;
+      }
+      v[u] = *reinterpret_cast<const float4*>(so + px * SROW + (dy * 2 + dx) * CS + j * 4);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (p.ex_x != nullptr) {
+#pragma unroll
+        for (int k = 0; k < PW_EX_KMAX; ++k) {
+          const float* wk = exw + k * CS + jq[u] * 4;
+          v[u].x = fmaf(xe[u][k], wk[0], v[u].x); v[u].y = fmaf(xe[u][k], wk[1], v[u].y);
+          v[u].z = fmaf(xe[u][k], wk[2], v[u].z); v[u].w = fmaf(xe[u][k], wk[3], v[u].w);
+        }
+      }
+      if (p.beta != 0.f) {
+        v[u].x += p.beta * old[u].x; v[u].y += p.beta * old[u].y; v[u].z += p.beta * old[u].z; v[u].w += p.beta * old[u].w;
+      }
+      if (p.mask_y != nullptr) {
+        v[u].x *= act_bwd_from_y(ym[u].x, p.mask_act); v[u].y *= act_bwd_from_y(ym[u].y, p.mask_act);
+        v[u].z *= act_bwd_from_y(ym[u].z, p.mask_act); v[u].w *= act_bwd_from_y(ym[u].w, p.mask_act);
+      }
+      reinterpret_cast<float4*>(p.out)[o4[u]] = v[u];
+    }
+  }
+}
+
 // K gradient channels, CS channels of the source whose gradient is produced (16: thread = pixel, all four taps;
 // 32: two threads per pixel, thread half h owns the taps of output row 2y + h -- a warp is uniform in h, so the
 // constant-memory operands stay warp-uniform).
@@ -993,17 +1063,12 @@ pwd2s_kernel(const PwdParams p) {
   constexpr int TP = PWD_THREADS / TPP;                            // gradient pixels per tile
   constexpr int NP = 4 * CS;                                       // outputs per gradient pixel
   constexpr int SROW = NP + 4;                                     // floats per staged pixel
-  constexpr int C4 = CS / 4;
   extern __shared__ __align__(16) float so[];                      // [TP][SROW]
   __shared__ float exw[PW_EX_KMAX * CS];
   const int tid = threadIdx.x;
   const int half = tid / TP, lp = tid - half * TP;                 // tap-row half, pixel inside the tile
-  for (int i = tid; i < PW_EX_KMAX * CS; i += PWD_THREADS)
-    exw[i] = (p.ex_x != nullptr && i < p.ex_K * CS)
-                 ? __ldg(p.ex_w + (long long)(i / CS) * p.ex_wk + (long long)(i % CS) * p.ex_wn) : 0.f;
+  pwd_load_exw<CS>(p, exw);
   __syncthreads();
-  const int Wout = 2 * p.Win;
-  const int wtile = p.Win < TP ? p.Win : TP;                       // lattice pixels per row inside a tile
   auto load_x = [&](uint32_t t, float4 (&xv)[K / 4]) {
     const float4* xr = reinterpret_cast<const float4*>(p.dz + ((size_t)t * TP + lp) * K);
 #pragma unroll
@@ -1045,55 +1110,7 @@ pwd2s_kernel(const PwdParams p) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) srow[j] = make_float4(acc[2 * j].x, acc[2 * j].y, acc[2 * j + 1].x, acc[2 * j + 1].y);
     __syncthreads();
-    // ---- coalesced output runs: per lattice row of the tile, rows 2*row and 2*row + 1 of the output, 2*wtile
-    // pixels of CS channels each.  TP*CS float4 per tile = 16 per thread, in batches of 4: every read-modify-write
-    // operand of a batch is requested before the first one is used ----
-    constexpr int PER_THREAD = TP * CS / PWD_THREADS;              // 16
-#pragma unroll 1
-    for (int b4 = 0; b4 < PER_THREAD / 4; ++b4) {
-      float4 v[4], old[4], ym[4];
-      float xe[4][PW_EX_KMAX];
-      size_t off[4];
-      int jq[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int f = tid + (b4 * 4 + u) * PWD_THREADS;            // float4 index inside the tile's outputs
-        const int j = f % C4;                                      // C4, 2 * wtile: powers of two
-        int r = f / C4;
-        const int ox = r & (2 * wtile - 1);
-        r >>= p.lw2;
-        const int dy = r & 1, lr = r >> 1;                         // output row parity, lattice row inside the tile
-        const int px = lr * wtile + (ox >> 1), dx = ox & 1;
-        jq[u] = j;
-        off[u] = (((size_t)(2 * (row0 + lr) + dy) * Wout + 2 * x0 + ox) * CS) + (size_t)j * 4;
-        if (p.beta != 0.f) old[u] = *reinterpret_cast<const float4*>(p.out + off[u]);
-        if (p.mask_y != nullptr) ym[u] = ld4(p.mask_y + off[u]);
-        if (p.ex_x != nullptr) {
-#pragma unroll
-          for (int k = 0; k < PW_EX_KMAX; ++k) xe[u][k] = k < p.ex_K ? __ldg(p.ex_x + (off[u] / CS) * p.ex_K + k) : 0.f;
-        }
-        v[u] = *reinterpret_cast<const float4*>(so + px * SROW + (dy * 2 + dx) * CS + j * 4);
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        if (p.ex_x != nullptr) {
-#pragma unroll
-          for (int k = 0; k < PW_EX_KMAX; ++k) {
-            const float* wk = exw + k * CS + jq[u] * 4;
-            v[u].x = fmaf(xe[u][k], wk[0], v[u].x); v[u].y = fmaf(xe[u][k], wk[1], v[u].y);
-            v[u].z = fmaf(xe[u][k], wk[2], v[u].z); v[u].w = fmaf(xe[u][k], wk[3], v[u].w);
-          }
-        }
-        if (p.beta != 0.f) {
-          v[u].x += p.beta * old[u].x; v[u].y += p.beta * old[u].y; v[u].z += p.beta * old[u].z; v[u].w += p.beta * old[u].w;
-        }
-        if (p.mask_y != nullptr) {
-          v[u].x *= act_bwd_from_y(ym[u].x, p.mask_act); v[u].y *= act_bwd_from_y(ym[u].y, p.mask_act);
-          v[u].z *= act_bwd_from_y(ym[u].z, p.mask_act); v[u].w *= act_bwd_from_y(ym[u].w, p.mask_act);
-        }
-        *reinterpret_cast<float4*>(p.out + off[u]) = v[u];
-      }
-    }
+    pwd_store_tile<TP, CS, SROW>(p, so, exw, row0, x0);
   }
 }
 
@@ -1113,21 +1130,38 @@ bool pwd2s_applicable(const GConvK& k, const float* bias, int act, const float* 
   if (k.ax.nt != k.Win || k.ay.nt != k.Hin || !pwd_pow2(k.Win) || k.M % TP != 0) return false;
   if (k.Win < TP && (TP % k.Win != 0 || ((long long)k.N * k.Hin) % (TP / k.Win) != 0)) return false;
   if (k.Hout != 2 * k.Hin || k.Wout != 2 * k.Win) return false;
+  if ((unsigned long long)k.M * k.cout_true >= (1ull << 32)) return false;      // float4 index of the output: 32 bits
   if (!aligned16(out) || (mask_y != nullptr && !aligned16(mask_y))) return false;
   if (ex != nullptr && (ex->K < 1 || ex->K > PW_EX_KMAX || ex->x == nullptr || ex->w == nullptr)) return false;
   return true;
 }
 
-template <int K, int CS>
-static int pwd2s_launch(const PwdParams& p0, cudaStream_t st) {
-  constexpr int TP = PWD_THREADS / (CS / 16);
-  PwdParams p = p0;
+// tile geometry of a launch with TP lattice pixels per tile (pwd2s_applicable checked that tiles cover whole rows or
+// row parts)
+static void pwd_tiling(PwdParams& p, int TP) {
   p.ntiles = p.M / TP;
   p.lwin = 0;
   while ((1 << p.lwin) < p.Win) ++p.lwin;
   const int w2 = 2 * (p.Win < TP ? p.Win : TP);
   p.lw2 = 0;
   while ((1 << p.lw2) < w2) ++p.lw2;
+}
+
+static PwdParams pwd_params(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, const PwExtra* ex) {
+  PwdParams p;
+  memset(&p, 0, sizeof(p));
+  p.dz = k.seg[0].ptr; p.K = k.seg[0].C; p.M = k.M; p.Win = k.Win;
+  p.beta = beta; p.mask_y = mask_y; p.mask_act = mask_act; p.out = out;
+  if (ex != nullptr) { p.ex_x = ex->x; p.ex_K = ex->K; p.ex_w = ex->w; p.ex_wk = ex->wk; p.ex_wn = ex->wn; }
+  p.w = k.w; p.wt = k.wt; p.wc = k.wc; p.wn = k.wn;
+  return p;
+}
+
+template <int K, int CS>
+static int pwd2s_launch(const PwdParams& p0, cudaStream_t st) {
+  constexpr int TP = PWD_THREADS / (CS / 16);
+  PwdParams p = p0;
+  pwd_tiling(p, TP);
   const size_t smem = (size_t)TP * (4 * CS + 4) * sizeof(float);
   int dev = 0;
   cudaGetDevice(&dev);
@@ -1155,13 +1189,154 @@ int launch_pwd2s(const GConvK& k, float beta, const float* mask_y, int mask_act,
   if (e == cudaSuccess)
     e = cudaMemcpyToSymbolAsync(pwd_cw, stage, (size_t)K * 2 * CS * sizeof(float2), 0, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwd weight table: %s", cudaGetErrorString(e));
-  PwdParams p;
-  memset(&p, 0, sizeof(p));
-  p.dz = k.seg[0].ptr; p.K = K; p.M = k.M; p.Win = k.Win;
-  p.beta = beta; p.mask_y = mask_y; p.mask_act = mask_act; p.out = out;
-  if (ex != nullptr) { p.ex_x = ex->x; p.ex_K = ex->K; p.ex_w = ex->w; p.ex_wk = ex->wk; p.ex_wn = ex->wn; }
+  const PwdParams p = pwd_params(k, beta, mask_y, mask_act, out, ex);
   if (CS == 16) return K == 16 ? pwd2s_launch<16, 16>(p, st) : pwd2s_launch<32, 16>(p, st);
   return K == 32 ? pwd2s_launch<32, 32>(p, st) : pwd2s_launch<64, 32>(p, st);
+}
+
+// =============================================================================================
+// The same depth-to-space input gradient on the tensor cores: per tile, the [TP x K] gradient rows times the
+// [K x 4*CS] weights as mma.sync m16n8k8 TF32 products with the 3xTF32 split of the wgmma kernels (activation hi
+// truncated or rounded per tc_rawhi, weights hi / lo rounded; three products, small terms first), so that the
+// product costs a few hundred tensor instructions per tile instead of the CUDA-core FMA stream of pwd2s_kernel.
+//   * weights: read once per CTA from the layer's kernel through the descriptor strides, split, and kept in shared
+//     memory in mma B-fragment order (one conflict-free LDS.128 per lane gives the hi and lo pair);
+//   * persistent grid of one wave; the gradient rows of the next tile are copied by cp.async into the second of two
+//     stages while this tile computes and stores;
+//   * tile = TP = 2048 / CS lattice pixels, 8 warps: warp = 16 pixels x 64 output columns;
+//   * the accumulators are staged in shared memory and leave through pwd_store_tile, the coalesced read-modify-write
+//     pass of pwd2s_kernel (beta, activation mask, fused pointwise term).
+// =============================================================================================
+template <int K, int CS>
+struct PwmCfg {
+  static constexpr int TP = 128 * 16 / CS;                        // lattice pixels per tile
+  static constexpr int MT = TP / 16;                              // m16 tiles per tile: warps per column group
+  static constexpr int NT = 4 * CS / 8;                           // n8 tiles of the [K x 4*CS] product
+  static constexpr int NTW = 8;                                   // n8 tiles per warp
+  static constexpr int XROW = K + 4;                              // staged gradient row (floats): conflict-free A loads
+  static constexpr int SROW = 4 * CS + 8;                         // staged output row (floats): conflict-free float2 stores
+  static constexpr size_t W_FLOATS = (size_t)K * 4 * CS * 2;
+  static constexpr size_t X_FLOATS = (size_t)TP * XROW;
+  static constexpr size_t SMEM = (W_FLOATS + 2 * X_FLOATS + (size_t)TP * SROW) * sizeof(float);
+  static_assert(MT * (NT / NTW) * 32 == PWD_THREADS, "one warp per 16 pixels x 64 columns");
+};
+
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], float b0, float b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(__float_as_uint(b0)), "r"(__float_as_uint(b1)));
+}
+
+template <int K, int CS>
+__global__ void __launch_bounds__(PWD_THREADS, 2)
+pwd2s_mma_kernel(const PwdParams p) {
+  using C = PwmCfg<K, CS>;
+  extern __shared__ __align__(16) float smem[];
+  float4* wf = reinterpret_cast<float4*>(smem);                   // [K/8][NT][lane]: (hi b0, hi b1, lo b0, lo b1)
+  float* xs = smem + C::W_FLOATS;                                 // 2 x [TP][XROW]
+  float* so = xs + 2 * C::X_FLOATS;                               // [TP][SROW]
+  __shared__ float exw[PW_EX_KMAX * CS];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int gq = lane >> 2, tq = lane & 3;                        // mma fragment row / column group of the lane
+
+  // B fragment of (k-step ks, n8 tile nt) for lane l: b0 = W[8ks + l%4][8nt + l/4], b1 = the same at k + 4
+  for (int i = tid; i < K / 8 * C::NT * 32; i += PWD_THREADS) {
+    const int l = i & 31, nt = (i >> 5) % C::NT, ks = (i >> 5) / C::NT;
+    const int n = 8 * nt + (l >> 2), k = 8 * ks + (l & 3);
+    const int tap = n / CS, c = n - tap * CS;
+    const float* w0 = p.w + tap * p.wt + k * p.wc + c * p.wn;
+    const float v0 = __ldg(w0), v1 = __ldg(w0 + 4 * p.wc);
+    const float h0 = tf32_rna(v0), h1 = tf32_rna(v1);
+    wf[i] = make_float4(h0, h1, tf32_rna(v0 - h0), tf32_rna(v1 - h1));
+  }
+  pwd_load_exw<CS>(p, exw);
+
+  auto stage = [&](uint32_t t, int buf) {                         // gradient rows of tile t: TP * K contiguous floats
+    const float4* src = reinterpret_cast<const float4*>(p.dz + (size_t)t * C::TP * K);
+    const uint32_t dst = pwx_smem_u32(xs + buf * C::X_FLOATS);
+#pragma unroll
+    for (int i = tid; i < C::TP * K / 4; i += PWD_THREADS) {
+      const int px = i / (K / 4), q = i % (K / 4);
+      cp_async16(dst + (px * C::XROW + 4 * q) * 4, src + i);
+    }
+  };
+  if (blockIdx.x < p.ntiles) stage(blockIdx.x, 0);
+  cp_async_commit();
+  const int mt = warp % C::MT, ng = warp / C::MT;                 // pixel rows 16 mt.., columns 64 ng..
+  int buf = 0;
+  for (uint32_t t = blockIdx.x; t < p.ntiles; t += gridDim.x, buf ^= 1) {
+    if (t + gridDim.x < p.ntiles) stage(t + gridDim.x, buf ^ 1);  // the other stage was last read before the staging barrier
+    cp_async_commit();
+    cp_async_wait<1>();
+    __syncthreads();                                              // tile t has landed; the previous tile's outputs are stored
+
+    float acc[C::NTW][4];
+#pragma unroll
+    for (int j = 0; j < C::NTW; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+    const float* xa = xs + buf * C::X_FLOATS + (16 * mt + gq) * C::XROW + tq;
+#pragma unroll 1
+    for (int ks = 0; ks < K / 8; ++ks) {                         // (unrolled, the B fragments of all k-steps are hoisted and spill)
+      uint32_t ah[4], al[4];
+      tf32_split(xa[8 * ks], p.rawhi, ah[0], al[0]);
+      tf32_split(xa[8 * C::XROW + 8 * ks], p.rawhi, ah[1], al[1]);
+      tf32_split(xa[8 * ks + 4], p.rawhi, ah[2], al[2]);
+      tf32_split(xa[8 * C::XROW + 8 * ks + 4], p.rawhi, ah[3], al[3]);
+#pragma unroll
+      for (int j = 0; j < C::NTW; ++j) {
+        const float4 b = wf[(ks * C::NT + ng * C::NTW + j) * 32 + lane];
+        mma_tf32(acc[j], al, b.x, b.y);                           // small terms first
+        mma_tf32(acc[j], ah, b.z, b.w);
+        mma_tf32(acc[j], ah, b.x, b.y);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < C::NTW; ++j) {
+      float* r0 = so + (16 * mt + gq) * C::SROW + 8 * (ng * C::NTW + j) + 2 * tq;
+      *reinterpret_cast<float2*>(r0) = make_float2(acc[j][0], acc[j][1]);
+      *reinterpret_cast<float2*>(r0 + 8 * C::SROW) = make_float2(acc[j][2], acc[j][3]);
+    }
+    __syncthreads();                                              // outputs staged; every read of stage buf is done
+    const uint32_t start = t * C::TP;
+    pwd_store_tile<C::TP, CS, C::SROW>(p, so, exw, start >> p.lwin, start & ((uint32_t)p.Win - 1u));
+  }
+}
+
+int g_opt_pwmma = -1;   // option "pwmma" / NLT_PWMMA: 1 (default) the tensor-core kernels of this file, 0 the FMA ones
+bool pwmma_enabled() {
+  if (g_opt_pwmma < 0) { const char* e = getenv("NLT_PWMMA"); g_opt_pwmma = (e && e[0] == '0') ? 0 : 1; }
+  return g_opt_pwmma == 1;
+}
+
+template <int K, int CS>
+static int pwd2s_mma_launch(const PwdParams& p0, cudaStream_t st) {
+  using C = PwmCfg<K, CS>;
+  PwdParams p = p0;
+  pwd_tiling(p, C::TP);
+  int dev = 0;
+  cudaGetDevice(&dev);
+  static int per_sm[64] = {0};                                    // resident CTAs per SM, per device
+  int& n = per_sm[dev >= 0 && dev < 64 ? dev : 0];
+  if (n == 0) {
+    cudaError_t e = cudaFuncSetAttribute(pwd2s_mma_kernel<K, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM);
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, pwd2s_mma_kernel<K, CS>, PWD_THREADS, C::SMEM);
+    if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwd2s_mma_kernel attributes: %s", cudaGetErrorString(e));
+    if (n < 1) return set_err(NLT_ERR_CUDA, "pwd2s_mma_kernel: no CTA fits on an SM");
+  }
+  const unsigned wave = (unsigned)sm_count() * (unsigned)n;
+  const unsigned grid = p.ntiles < wave ? p.ntiles : wave;
+  pwd2s_mma_kernel<K, CS><<<grid, PWD_THREADS, C::SMEM, st>>>(p);
+  NLT_CUDA_LAUNCH_CHECK("pwd2s_mma_kernel");
+  return NLT_OK;
+}
+
+int launch_pwd2s_mma(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
+                     const PwExtra* ex) {
+  const int K = k.seg[0].C, CS = k.cout_true;
+  PwdParams p = pwd_params(k, beta, mask_y, mask_act, out, ex);
+  if (g_opt_tc_rawhi < 0) { const char* e = getenv("NLT_TC_RAWHI"); g_opt_tc_rawhi = (e && e[0] == '0') ? 0 : 1; }
+  p.rawhi = g_opt_tc_rawhi;
+  if (CS == 16) return K == 16 ? pwd2s_mma_launch<16, 16>(p, st) : pwd2s_mma_launch<32, 16>(p, st);
+  return K == 32 ? pwd2s_mma_launch<32, 32>(p, st) : pwd2s_mma_launch<64, 32>(p, st);
 }
 
 // =============================================================================================

@@ -199,25 +199,6 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
   return d;
 }
 
-__device__ __forceinline__ float tf32_rna(float x) {
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-  return __uint_as_float(r);
-}
-// Round-to-nearest TF32 in two integer instructions (cvt.rna.tf32 expands to several instructions with its inf/nan
-// handling).  Adding half an ulp to the bit pattern and clearing the low 13 mantissa bits rounds the magnitude to
-// nearest (ties away), carries into the exponent correctly, and is only wrong for inf/nan, which the split does not
-// need to preserve.
-__device__ __forceinline__ float tf32_round(float x) {
-  return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-}
-// 3xTF32 split of one activation: hi = x truncated (rawhi) or rounded to TF32; lo = x - hi (exact), rounded to TF32
-__device__ __forceinline__ void tf32_split(float x, int rawhi, uint32_t& hi, uint32_t& lo) {
-  const float h = rawhi ? __uint_as_float(__float_as_uint(x) & 0xFFFFE000u) : tf32_round(x);
-  hi = __float_as_uint(h);
-  lo = __float_as_uint(tf32_round(x - h));
-}
-
 // ---------------------------------------------------------------------------------------------
 // weight pack: Bhi/Blo [kb][Cout_pad][KBW] (K-major rows), TF32-rounded split
 // ---------------------------------------------------------------------------------------------
