@@ -83,9 +83,11 @@ GEOMS = [
     ('deconv', 2, 1, 32, 16, [16], 16),
     ('conv', 2, 2, 64, 64, [32, 16], 32),       # mixed 32/16 sources -> 16-wide blocks
     # wide pointwise conv into 16 channels (nlt_pwx.cu: level 0 of the 64-channel query stack): cp.async-staged
-    # 256-pixel tiles, ragged last tile, float4-able and scalar sources mixed, K not a multiple of 32
-    ('conv', 2, 2, 8, 512, [16, 16], 32),       # its input gradients: depth-to-space K = 32 -> 4 x 16 (pwd2s kernel)
-    ('conv', 2, 2, 16, 256, [32], 64),          # pwd2s with 32-channel sources (two threads per gradient pixel), K = 64
+    # 256-pixel tiles, ragged last tile, float4-able and scalar sources mixed, K not a multiple of 32.
+    # The depth-to-space input gradients of the next five shapes run on pwd2s_mma_kernel (tc = 1 and pwmma = 1, the
+    # defaults) and on pwd2s_kernel with tc = 0 or pwmma = 0
+    ('conv', 2, 2, 8, 512, [16, 16], 32),       # its input gradients: depth-to-space K = 32 -> 4 x 16
+    ('conv', 2, 2, 16, 256, [32], 64),          # 32-channel sources (pwd2s_kernel: two threads per pixel), K = 64
     ('conv', 2, 2, 32, 128, [32, 32], 64),      # ... lattice rows narrower than a tile: two rows per tile
     ('conv', 2, 2, 32, 128, [16], 16),          # ... four lattice rows per tile, 16-channel source
     ('conv', 2, 2, 32, 128, [32], 32),          # K = 32 -> 4 x 32
