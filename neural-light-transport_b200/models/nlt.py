@@ -23,18 +23,25 @@ from networks import convnet
 from .base import Model as BaseModel
 
 
-def _dev_tensor(x, device):
+def _dev_tensor(x, device, out=None):
     """Moves a batch element to the device as contiguous fp32 (inputs may be
     pinned host tensors: the H2D copy is part of the end-to-end path).
     uint8 tensors are image samples still in PNG units: they cross PCIe as bytes and become v / 255 on the device
-    (bit-identical to the host pipeline's float32(v / 255.0); datasets with `uint8_inputs = True` emit them)."""
+    (bit-identical to the host pipeline's float32(v / 255.0); datasets with `uint8_inputs = True` emit them).
+    `out`: a contiguous fp32 device tensor of the same shape to write into (the static inputs of a CUDA graph)."""
     if not torch.is_tensor(x):
         x = torch.as_tensor(np.asarray(x))
+    if out is not None and (tuple(out.shape) != tuple(x.shape) or out.dtype != torch.float32 or not out.is_contiguous()):
+        raise ValueError('batch element of shape %s / %s does not fit the fp32 buffer %s' % (
+            tuple(x.shape), x.dtype, tuple(out.shape)))
     if x.dtype == torch.uint8:
         xd = x.to(device=device, non_blocking=True).contiguous()
-        out = torch.empty(xd.shape, dtype=torch.float32, device=device)
+        if out is None:
+            out = torch.empty(xd.shape, dtype=torch.float32, device=device)
         nat.check(nat.lib().nlt_u8_to_f32(xd.data_ptr(), xd.numel(), nat.ptr(out), nat.stream()))
         return out
+    if out is not None:
+        return out.copy_(x, non_blocking=True)
     if x.device != device or x.dtype != torch.float32:
         x = x.to(device=device, dtype=torch.float32, non_blocking=True)
     return x.contiguous()

@@ -247,9 +247,11 @@ class GraphedTrainStep:
 
     def _capture(self, batch):
         import engine
+        from models.nlt import _dev_tensor
         dev = self.model.device
-        self.static_batch = tuple(t.to(dev, torch.float32).contiguous().clone() if torch.is_tensor(t) else t
-                                  for t in batch)
+        # uint8 image tensors become v / 255 here, as in the eager step (models/nlt.py:_dev_tensor)
+        self.static_batch = tuple(_dev_tensor(t, dev, out=torch.empty(t.shape, dtype=torch.float32, device=dev))
+                                  if torch.is_tensor(t) else t for t in batch)
         with engine.use_workspaces(*self._ws):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
@@ -291,9 +293,10 @@ class GraphedTrainStep:
         if self.graph is None:
             self._capture(batch)
         if batch is not self.static_batch:
+            from models.nlt import _dev_tensor
             for dst, src in zip(self.static_batch, batch):
                 if torch.is_tensor(dst):
-                    dst.copy_(src, non_blocking=True)
+                    _dev_tensor(src, dst.device, out=dst)     # uint8 -> v / 255, like the eager step
         self.graph.replay()
         if self.full_step_in_graph:
             self.optimizer.iterations += 1       # host mirror of the device step counter
