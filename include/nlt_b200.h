@@ -201,6 +201,23 @@ int nlt_l2_loss(const float* pred, const float* gt, int32_t B,
                 int64_t per_sample, float loss_scale, float* loss,
                 float* d_pred, void* workspace, void* stream);
 
+/* losses.L1 (nlt/losses.py:27-36, MeanAbsoluteError then reduce_mean) per sample, fused with its gradient:
+ *   loss[b] = mean_{h,w,c} |pred - gt| ;  d_pred = sign(pred - gt) * loss_scale / per_sample (exactly 0 on ties)
+ * d_pred may be NULL.  Deterministic (per-block partials, fixed-order sum in double).
+ * workspace: >= nlt_l1_loss_workspace_bytes() (< 0 for B <= 0 or per_sample <= 0). */
+int64_t nlt_l1_loss_workspace_bytes(int32_t B, int64_t per_sample);
+int nlt_l1_loss(const float* pred, const float* gt, int32_t B, int64_t per_sample, float loss_scale, float* loss,
+                float* d_pred, void* workspace, void* stream);
+
+/* losses.SSIM (nlt/losses.py:75-87) per sample, fused with its gradient: tf.image.ssim(gt, pred, max_val) of TF 2.2
+ * (11 x 11 Gaussian window, sigma 1.5, VALID, k1 = 0.01, k2 = 0.03), averaged over channels and output pixels:
+ *   loss[b] = (1 - ssim_b) / 2 ;  d_pred = d(sum_b loss[b] * loss_scale) / d(pred)
+ * pred, gt: [B,H,W,3] with H, W >= 11 and B <= 65535; d_pred may be NULL (the loss is bit-identical either way).
+ * Deterministic.  workspace: >= nlt_ssim_loss_workspace_bytes() (< 0 for B <= 0, H < 11 or W < 11). */
+int64_t nlt_ssim_loss_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int nlt_ssim_loss(const float* pred, const float* gt, int32_t B, int32_t H, int32_t W, float max_val, float loss_scale,
+                  float* loss, float* d_pred, void* workspace, void* stream);
+
 /* SURVEY 8f row N1 (checked on the CPU and on hardware against the oracle pinned to the reference's wavelet
  * fixtures): losses.Barron with keep_batch (nlt/losses.py:90-121) fused with its gradient.
  *   r = (gt - pred) [* alpha]  ->  volume-preserving YUV  ->  `levels`-level CDF 9/7 analysis (reflecting

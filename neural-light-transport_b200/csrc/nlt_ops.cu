@@ -1,6 +1,6 @@
 // HBM-bound streaming kernels around the conv stack: observation mean,
 // UV->camera tail (base add, corner zero, bilinear resample, alpha blend) and
-// its scatter-add backward, bilinear resize, fused L2 loss + gradient, fused
+// its scatter-add backward, bilinear resize, fused L2 / L1 loss + gradient, fused
 // AMSGrad.  All of these are byte movers: vectorised where alignment allows,
 // grids sized in multiples of the SM count with grid-stride loops.
 #include "nlt_common.cuh"
@@ -358,6 +358,61 @@ __global__ void l2_final_kernel(const float* __restrict__ partial, int B, int nb
 }
 
 // ---------------------------------------------------------------------------
+// L1 loss (keep_batch) + gradient -- nlt/losses.py:27-36 (MeanAbsoluteError, then reduce_mean)
+// Same grid as the L2 pair.  d_pred = sign(pred - gt) * dscale, exactly 0 on ties (TF's Abs gradient).
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ float l1_grad(float d, float dscale) {
+  return d > 0.f ? dscale : (d < 0.f ? -dscale : d * dscale);    // d * dscale: 0 on ties, NaN stays NaN
+}
+
+__global__ void l1_partial_kernel(const float* __restrict__ pred, const float* __restrict__ gt, size_t per_sample,
+                                  float dscale, float* __restrict__ partial, float* __restrict__ d_pred) {
+  const int b = blockIdx.y;
+  const float* pp = pred + (size_t)b * per_sample;
+  const float* gg = gt + (size_t)b * per_sample;
+  float* dp = d_pred ? d_pred + (size_t)b * per_sample : nullptr;
+  float s = 0.f;
+  if ((per_sample & 3) == 0 && ((((uintptr_t)pp) | ((uintptr_t)gg) | ((uintptr_t)dp)) & 15) == 0) {
+    const float4* p4 = reinterpret_cast<const float4*>(pp);
+    const float4* g4 = reinterpret_cast<const float4*>(gg);
+    float4* d4 = reinterpret_cast<float4*>(dp);
+    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+    const size_t n4 = per_sample >> 2;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+      const float4 a = __ldg(p4 + i), b4 = __ldg(g4 + i);
+      const float4 d = make_float4(a.x - b4.x, a.y - b4.y, a.z - b4.z, a.w - b4.w);
+      s0 += fabsf(d.x); s1 += fabsf(d.y); s2 += fabsf(d.z); s3 += fabsf(d.w);
+      if (dp) d4[i] = make_float4(l1_grad(d.x, dscale), l1_grad(d.y, dscale), l1_grad(d.z, dscale), l1_grad(d.w, dscale));
+    }
+    s = (s0 + s1) + (s2 + s3);
+  } else {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < per_sample; i += (size_t)gridDim.x * blockDim.x) {
+      const float d = __ldg(pp + i) - __ldg(gg + i);
+      s += fabsf(d);
+      if (dp) dp[i] = l1_grad(d, dscale);
+    }
+  }
+  __shared__ float red[L2_THREADS];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = L2_THREADS / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) partial[(size_t)b * gridDim.x + blockIdx.x] = red[0];
+}
+
+__global__ void l1_final_kernel(const float* __restrict__ partial, int B, int nblk, double inv_n,
+                                float* __restrict__ loss) {
+  // one thread per sample, fixed summation order in double -> deterministic
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  double s = 0.0;
+  for (int i = 0; i < nblk; ++i) s += partial[(size_t)b * nblk + i];
+  loss[b] = (float)(s * inv_n);
+}
+
+// ---------------------------------------------------------------------------
 // AMSGrad -- tf.keras.optimizers.Adam(amsgrad=True), nlt/trainvali.py:122-127
 // ---------------------------------------------------------------------------
 __global__ void amsgrad_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
@@ -556,6 +611,25 @@ int nlt_l2_loss(const float* pred, const float* gt, int32_t B, int64_t per_sampl
   NLT_CUDA_LAUNCH_CHECK("l2_partial_kernel");
   l2_final_kernel<<<(B + 31) / 32, 32, 0, st>>>(partial, B, L2_BLOCKS_PER_SAMPLE, 1.f / (float)per_sample, loss);
   NLT_CUDA_LAUNCH_CHECK("l2_final_kernel");
+  return NLT_OK;
+}
+
+int64_t nlt_l1_loss_workspace_bytes(int32_t B, int64_t per_sample) {
+  if (B <= 0 || per_sample <= 0) return -1;
+  return (int64_t)B * L2_BLOCKS_PER_SAMPLE * sizeof(float);
+}
+
+int nlt_l1_loss(const float* pred, const float* gt, int32_t B, int64_t per_sample, float loss_scale, float* loss,
+                float* d_pred, void* workspace, void* stream) {
+  NLT_CHECK_ARG(pred && gt && loss && workspace && B > 0 && B <= 65535 && per_sample > 0, "l1_loss: bad argument");
+  cudaStream_t st = (cudaStream_t)stream;
+  float* partial = (float*)workspace;
+  const float dscale = (float)((double)loss_scale / (double)per_sample);
+  dim3 grid(L2_BLOCKS_PER_SAMPLE, B);
+  l1_partial_kernel<<<grid, L2_THREADS, 0, st>>>(pred, gt, (size_t)per_sample, dscale, partial, d_pred);
+  NLT_CUDA_LAUNCH_CHECK("l1_partial_kernel");
+  l1_final_kernel<<<(B + 31) / 32, 32, 0, st>>>(partial, B, L2_BLOCKS_PER_SAMPLE, 1.0 / (double)per_sample, loss);
+  NLT_CUDA_LAUNCH_CHECK("l1_final_kernel");
   return NLT_OK;
 }
 

@@ -1,7 +1,7 @@
 """Losses with the reference's class names (nlt/losses.py).
 
-L2 (SURVEY.md 8a a10: the loss used when timing the path) and Barron (row N1: the
-first term of the shipped `loss = barron,1e+0lpips`) are each fused with their own
+L2 (SURVEY.md 8a a10: the loss used when timing the path), L1, SSIM and Barron (row N1:
+the first term of the shipped `loss = barron,1e+0lpips`) are each fused with their own
 gradient in CUDA.  LPIPS (the second term) raises NotImplementedError.
 """
 import torch
@@ -42,13 +42,74 @@ class L2():
 
 
 class L1():
-    def __call__(self, gt, pred, weights=None):
-        raise NotImplementedError('l1 is not on the accelerated path')
+    """nlt/losses.py:27-36 -- mean absolute error; keep_batch -> (N,), fused with its gradient (nlt_l1_loss).
+    The reference's L1 takes no keep_batch (DESIGN.md section 1, difference (vi)); keep_batch=False gives its scalar."""
+
+    def __init__(self):
+        self._ws = None
+        self.d_pred = None
+        self.grad_scale = None
+
+    def __call__(self, gt, pred, keep_batch=False, weights=None):
+        if weights is not None:
+            raise NotImplementedError('sample weights')
+        lib = nat.lib()
+        B = pred.shape[0]
+        per = pred.numel() // B
+        need = lib.nlt_l1_loss_workspace_bytes(B, per)
+        if need < 0:
+            nat.check(-1)
+        if self._ws is None or self._ws.numel() * 4 < need or self._ws.device != pred.device:
+            self._ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=pred.device)
+        loss = torch.empty(B, dtype=torch.float32, device=pred.device)
+        want_grad = self.grad_scale is not None
+        self.d_pred = torch.empty_like(pred) if want_grad else None
+        scale = float(self.grad_scale) if want_grad else 0.0
+        if not keep_batch and want_grad:
+            scale = scale / B
+        from engine import PROF
+        PROF.run('fwd loss l1', 4 * pred.numel() * (3 if want_grad else 2), lambda: nat.check(lib.nlt_l1_loss(
+            nat.ptr(pred), nat.ptr(gt), B, per, scale, nat.ptr(loss), nat.ptr(self.d_pred), nat.ptr(self._ws),
+            nat.stream())))
+        return loss if keep_batch else loss.mean()
 
 
 class SSIM():
+    """nlt/losses.py:75-87 -- (1 - tf.image.ssim(gt, pred, dynamic_range)) / 2 per sample; keep_batch -> (N,), fused
+    with its gradient (nlt_ssim_loss).  The reference's SSIM takes no keep_batch (DESIGN.md section 1, difference
+    (vi)); keep_batch=False gives its scalar.  Images need at least 11 x 11 pixels (the window, VALID)."""
+    WIN = 11
+
     def __init__(self, dynamic_range):
-        raise NotImplementedError('ssim is not on the accelerated path')
+        self.dynamic_range = float(dynamic_range)
+        self._ws = None
+        self.d_pred = None
+        self.grad_scale = None
+
+    def __call__(self, gt, pred, keep_batch=False, weights=None):
+        if weights is not None:
+            raise NotImplementedError('sample weights')
+        B, H, W, C3 = pred.shape
+        if C3 != 3 or H < self.WIN or W < self.WIN or tuple(gt.shape) != tuple(pred.shape):
+            raise ValueError('ssim: expected two [N, H >= %d, W >= %d, 3] images, got %s and %s' % (
+                self.WIN, self.WIN, tuple(gt.shape), tuple(pred.shape)))
+        lib = nat.lib()
+        need = lib.nlt_ssim_loss_workspace_bytes(B, H, W)
+        if need < 0:
+            nat.check(-1)
+        if self._ws is None or self._ws.numel() * 4 < need or self._ws.device != pred.device:
+            self._ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=pred.device)
+        loss = torch.empty(B, dtype=torch.float32, device=pred.device)
+        want_grad = self.grad_scale is not None
+        self.d_pred = torch.empty_like(pred) if want_grad else None
+        scale = float(self.grad_scale) if want_grad else 0.0
+        if not keep_batch and want_grad:
+            scale = scale / B
+        from engine import PROF
+        PROF.run('fwd loss ssim', 4 * pred.numel() * (3 if want_grad else 2), lambda: nat.check(lib.nlt_ssim_loss(
+            nat.ptr(pred), nat.ptr(gt), B, H, W, self.dynamic_range, scale, nat.ptr(loss), nat.ptr(self.d_pred),
+            nat.ptr(self._ws), nat.stream())))
+        return loss if keep_batch else loss.mean()
 
 
 class Barron():

@@ -82,6 +82,11 @@ _SIGS = {
     'nlt_l2_loss_workspace_bytes': (C.c_int64, [C.c_int32, C.c_int64]),
     'nlt_l2_loss': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
                               C.c_void_p, C.c_void_p]),
+    'nlt_l1_loss_workspace_bytes': (C.c_int64, [C.c_int32, C.c_int64]),
+    'nlt_l1_loss': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_void_p]),
+    'nlt_ssim_loss_workspace_bytes': (C.c_int64, [C.c_int32] * 3),
+    'nlt_ssim_loss': (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_float] * 2 + [C.c_void_p] * 4),
     'nlt_amsgrad_step': (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int32] + [C.c_float] * 5 + [C.c_void_p]),
     'nlt_amsgrad_step_dev': (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_void_p] + [C.c_float] * 5 + [C.c_void_p]),
     'nlt_pixelnorm_fwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int, C.c_void_p, C.c_void_p]),
