@@ -255,6 +255,26 @@ int nlt_instnorm_bwd(const float* x, const float* dz, const float* gamma, const 
                      int32_t N, int32_t HW, int32_t C, float* dx, float* dgamma, float* dbeta, int accumulate,
                      void* workspace, void* stream);
 
+/* The U-Net ops of `pool = max | avg` (nlt/networks/convnet.py:50-80).  x, y, d_x, d_y: [N,H,W,C] NHWC (any C; float4
+ * rows when C % 4 == 0 and the pointers are 16-byte aligned).  Deterministic: no atomics.
+ *   pool2x2      tf.keras.layers.{Max,Average}Pooling2D(2, 2, 'same') (elements.py:81-94): y [N,ceil(H/2),ceil(W/2),C];
+ *                odd sizes clip the window at the right / bottom edge, avg divides by the valid taps.
+ *                _bwd: d_x = (beta * d_x + g) * act'(mask_y), g = the window's d_y routed to the FIRST maximum of the
+ *                window in row-major tap order (recomputed from x; 0 at the other taps) for max, d_y / valid taps for
+ *                avg.  mask_y may be NULL; beta is 0 or 1.
+ *   upsample2x   tf.keras.layers.UpSampling2D(2, interpolation='bilinear') (elements.py:42-48) = tf.image.resize to
+ *                (2H, 2W), half-pixel centres: y [N,2H,2W,C].  A batch-1 x gives a batch-1 y (broadcast segment).
+ *                _bwd: the exact adjoint, gathered per low-resolution pixel (<= 4 x 4 taps of d_y [N,2H,2W,C]),
+ *                with the same beta / mask epilogue into d_x [N,H,W,C]. */
+#define NLT_POOL_MAX 0
+#define NLT_POOL_AVG 1
+int nlt_pool2x2_fwd(const float* x, int32_t N, int32_t H, int32_t W, int32_t C, int kind, float* y, void* stream);
+int nlt_pool2x2_bwd(const float* x, const float* d_y, int32_t N, int32_t H, int32_t W, int32_t C, int kind, float beta,
+                    const float* mask_y, int mask_act, float* d_x, void* stream);
+int nlt_upsample2x_bilinear_fwd(const float* x, int32_t N, int32_t H, int32_t W, int32_t C, float* y, void* stream);
+int nlt_upsample2x_bilinear_bwd(const float* d_y, int32_t N, int32_t H, int32_t W, int32_t C, float beta,
+                                const float* mask_y, int mask_act, float* d_x, void* stream);
+
 /* uint8 image samples -> float32 in [0, 1] (v / 255, correctly rounded = the host pipeline's
  * float32(v / 255.0), nlt/datasets/nlt.py:134-139): lets a batch cross PCIe as bytes (SURVEY 8f N3). */
 int nlt_u8_to_f32(const uint8_t* in, int64_t n, float* out, void* stream);

@@ -613,6 +613,77 @@ class NormLayer:
         out.grad = None
 
 
+class PoolLayer:
+    """`pool(type)` at the end of a down block (nlt/networks/elements.py:81-94, convnet.py:58): 2x2 / stride-2 'same'
+    max or average pooling.  The output carries no activation; the backward pass makes one contribution into its
+    input, which applies that input's activation mask.  The max argmax is recomputed from the input, which is kept
+    anyway as the mask source, so nothing new is stored."""
+    KINDS = {'max': 0, 'avg': 1}          # NLT_POOL_MAX / NLT_POOL_AVG
+
+    def __init__(self, kind):
+        assert kind in self.KINDS
+        self.kind = kind
+        self.name = kind + 'pool'
+
+    def forward(self, x, tape=None):
+        lib = nat.lib()
+        t = x.t
+        N, H, W, C = t.shape
+        y = torch.empty((N, (H + 1) // 2, (W + 1) // 2, C), dtype=torch.float32, device=t.device)
+        code = self.KINDS[self.kind]
+        PROF.run('fwd ' + self.name, 4 * (t.numel() + y.numel()), lambda: nat.check(
+            lib.nlt_pool2x2_fwd(nat.ptr(t), N, H, W, C, code, nat.ptr(y), nat.stream())))
+        out = Act(y, act=None, needs_grad=tape is not None and x.needs_grad)
+        if tape is not None and x.needs_grad:
+            x.n_cons += 1
+
+            def bwd():
+                settle(out)
+                dy = out.grad
+                if dy is None:
+                    return
+
+                def write(o, beta, mask, mask_act, term=None):
+                    nb = 4 * (dy.numel() + o.numel() * (2 + (beta != 0) + (mask is not None)))
+                    PROF.run('dgrad ' + self.name, nb, lambda: nat.check(lib.nlt_pool2x2_bwd(
+                        nat.ptr(t), nat.ptr(dy), N, H, W, C, code, beta, nat.ptr(mask), mask_act, nat.ptr(o),
+                        nat.stream())))
+                contribute(x, write)
+                out.grad = None
+            tape.record(bwd)
+        return out
+
+
+def upsample2x(a, tape=None):
+    """UpSampling2D(2, 'bilinear') of one Act (the first half of `upconv`, nlt/networks/elements.py:42-48).  A batch-1
+    broadcast source stays batch 1.  The result's gradient accumulates from every segment that reads it; its backward
+    pass then makes one contribution into the source."""
+    lib = nat.lib()
+    t = a.t
+    N, H, W, C = t.shape
+    y = torch.empty((N, 2 * H, 2 * W, C), dtype=torch.float32, device=t.device)
+    PROF.run('fwd upsample2x', 4 * (t.numel() + y.numel()), lambda: nat.check(
+        lib.nlt_upsample2x_bilinear_fwd(nat.ptr(t), N, H, W, C, nat.ptr(y), nat.stream())))
+    out = Act(y, act=None, needs_grad=tape is not None and a.needs_grad)
+    if tape is not None and a.needs_grad:
+        a.n_cons += 1
+
+        def bwd():
+            settle(out)
+            dy = out.grad
+            if dy is None:
+                return
+
+            def write(o, beta, mask, mask_act, term=None):
+                nb = 4 * (dy.numel() + o.numel() * (1 + (beta != 0) + (mask is not None)))
+                PROF.run('dgrad upsample2x', nb, lambda: nat.check(lib.nlt_upsample2x_bilinear_bwd(
+                    nat.ptr(dy), N, H, W, C, beta, nat.ptr(mask), mask_act, nat.ptr(o), nat.stream())))
+            contribute(a, write)
+            out.grad = None
+        tape.record(bwd)
+    return out
+
+
 def kmean(obs_y, K, tape=None, weights=None):
     """mean over the K stacked observations (nlt/models/nlt.py:161-164).
     obs_y: Act [K*B,H,W,C] (k-major).  K == 1 aliases (no kernel, no copy)."""

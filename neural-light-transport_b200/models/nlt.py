@@ -127,6 +127,8 @@ class Model(BaseModel):
                 for ci, nm in enumerate(blk.norms):
                     if nm is not None and not nm.has_params:
                         nm.name = '%s.%d.%d.norm %snorm %d' % (net, li, ci, nm.kind, nm.cout)
+                if getattr(blk, 'pool', None) is not None:
+                    blk.pool.name = '%s.%d.pool %spool %d' % (net, li, blk.pool.kind, blk.convs[-1].cout)
 
     @property
     def trainable_variables(self):
@@ -189,6 +191,7 @@ class Model(BaseModel):
             nn_rgb, nn_rgb_camspc = batch  # *rgb* are placeholders for testing
         if self.device is None:
             raise nat.NativeError('no CUDA device: the NLT hot path has no CPU fallback')
+        self._check_uv_size(base.shape[1], base.shape[2])
         dev = self.device
         base, cvis, lvis, warp = (_dev_tensor(t, dev) for t in (base, cvis, lvis, warp))
         # The reference passes exactly one neighbour (nlt.py:96, "only one neighbor") while `_call` takes a list of
@@ -290,6 +293,7 @@ class Model(BaseModel):
 
     def _call(self, query_x, obs_xs, obs_weights=None, obs_override=None):
         """Reference signature (nlt.py:141): tensors in, tensor out."""
+        self._check_uv_size(query_x.shape[1], query_x.shape[2])
         dev = self.device
         q = [Seg(Act(_dev_tensor(query_x, dev)))]
         K = len(obs_xs)
@@ -298,6 +302,14 @@ class Model(BaseModel):
         if obs_weights is not None:
             obs_weights = _dev_tensor(obs_weights, dev).reshape(obs.shape[0] // K, K)
         return self._call_segs(q, [Seg(Act(obs))], K, obs_weights, obs_override, None).t
+
+    def _check_uv_size(self, H, W):
+        """With `pool` set every down block halves the UV map and the decoder concatenates each level's skip tensor at
+        the same size, so H and W must be multiples of 2**(down blocks).  Raised before anything reaches the device."""
+        n = sum(1 for blk in self.net['query'].layers if getattr(blk, 'pool', None) is not None)
+        if n and (int(H) % (1 << n) or int(W) % (1 << n)):
+            raise ValueError('pool=%s: the UV size %dx%d is not a multiple of 2**%d = %d (one halving per down block)'
+                             % (self.net['query'].layers[1].pool.kind, int(H), int(W), n, 1 << n))
 
     def _call_segs(self, query_x, obs_x, K, obs_weights, obs_override, tape):
         """The two-stream U-Net walk of nlt.py:141-199 over virtual concats.

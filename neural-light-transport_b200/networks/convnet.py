@@ -5,20 +5,24 @@ on engine segments), which is what `nlt_test.extract_feat` and the two-stream wa
 import numpy as np
 import torch
 
-from engine import Act, Seg
+from engine import Act, Seg, upsample2x
 from util import net as netutil
 from .seq import Network as BaseNetwork
-from .elements import conv, norm, act, pool, deconv, NormLayer
+from .elements import conv, norm, act, pool, deconv, upconv, NormLayer
 
 
 class Block:
     """One entry of Network.layers: 1x1 conv, down block or up block, run as fused conv(+bias+act) CUDA ops; with
     `norm != None` every conv of a two-conv block is followed by an engine.NormLayer that carries the activation
-    (conv -> norm -> act, nlt/networks/convnet.py:50-59, 67-76)."""
+    (conv -> norm -> act, nlt/networks/convnet.py:50-59, 67-76).  With `pool != None` a down block ends in an
+    engine.PoolLayer and an up block starts with `upconv`: bilinear x2 of every distinct source of its input concat,
+    then convs[0], a linear 2x2 conv (convnet.py:58, 67)."""
 
-    def __init__(self, convs, norms=None):
+    def __init__(self, convs, norms=None, pool=None, upconv=False):
         self.convs = convs
         self.norms = norms if norms is not None else [None] * len(convs)
+        self.pool = pool
+        self.upconv = upconv
 
     @property
     def built(self):
@@ -44,12 +48,30 @@ class Block:
 
     def forward_segs(self, segs, tape=None):
         """segs: list of engine.Seg (virtual concat) -> engine.Act"""
+        if self.upconv:
+            segs = self._upsample(segs, tape)
         y = None
         for i, (c, nm) in enumerate(zip(self.convs, self.norms)):
             y = c.forward(segs if i == 0 else [Seg(y)], tape)
             if nm is not None:
                 y = nm.forward(y, tape)
+        if self.pool is not None:
+            y = self.pool.forward(y, tape)
         return y
+
+    @staticmethod
+    def _upsample(segs, tape):
+        """Each distinct source Act is upsampled once: the first up block reads [q, agg, q, agg] (the bottleneck
+        concatenated with itself), which costs two upsamples, and the conv reads each result twice."""
+        done = {}
+        out = []
+        for sg in segs:
+            if sg.sub is not None:
+                raise ValueError('upconv: a segment with a subtrahend cannot be upsampled')
+            if id(sg.a) not in done:
+                done[id(sg.a)] = upsample2x(sg.a, tape)
+            out.append(Seg(done[id(sg.a)], bcast=sg.bcast))
+        return out
 
     def __call__(self, x):
         if isinstance(x, Act):
@@ -71,19 +93,26 @@ def _block_kinds(n_feat):
 class Network(BaseNetwork):
     """Constructor signature, `.layers`, `.is_contracting` and `.spatsize_changes` of nlt/networks/convnet.py:30-90:
     [1x1 conv -> depth0] + one two-conv block per schedule entry (strided conv + conv when contracting, strided
-    transposed conv + transposed conv when expanding, each followed by the activation) + [1x1 conv -> 3]."""
+    transposed conv + transposed conv when expanding, each followed by the activation) + [1x1 conv -> 3].
+    `pool_type = max | avg` gives the classic U-Net: every down block ends in a 2x2 pool and every up block starts with
+    `upconv(n)`.  Only `stride = 1` is accepted with a pool: at stride 2 each level shrinks by 4, and six levels would
+    need UV sizes that are multiples of 4**6 for the reference's own skip concat (nlt/models/nlt.py:190)."""
 
     def __init__(self, depth0, depth, kernel, stride, norm_type=None, act_type='relu', pool_type=None):
         super().__init__()
         # unsupported normalisation / pooling kinds raise NotImplementedError right here, like the reference's
         # element factories; the supported kind for both is None (identity)
         norm_kind = norm(self.str2none(norm_type))
-        pool(self.str2none(pool_type))
+        pool_kind = pool(self.str2none(pool_type))
         activation = act(act_type)
+        if pool_kind is not None and stride != 1:
+            raise NotImplementedError(
+                'pool=%s with stride=%d: every level would shrink the UV map by %d, so six levels need sizes that are '
+                'multiples of %d**6; pooling networks take stride=1' % (pool_type, stride, 2 * stride, 2 * stride))
         n_feat = netutil.gen_feat_n(depth0, depth)
 
-        def add(convs, contracting, scale, norms=None):
-            self.layers.append(Block(convs, norms))
+        def add(convs, contracting, scale, norms=None, **kw):
+            self.layers.append(Block(convs, norms, **kw))
             self.is_contracting.append(contracting)
             self.spatsize_changes.append(scale)
 
@@ -100,10 +129,18 @@ class Network(BaseNetwork):
         for kind, n in _block_kinds(n_feat):
             if kind == 'down':
                 convs, norms = pair(conv, n)
-                add(convs, True, 1 / stride, norms)
+                if pool_kind is None:
+                    add(convs, True, 1 / stride, norms)
+                else:
+                    add(convs, True, 1 / stride / 2, norms, pool=pool(self.str2none(pool_type)))
             else:
                 convs, norms = pair(deconv, n)
-                add(convs, False, stride, norms)
+                if pool_kind is None:
+                    add(convs, False, stride, norms)
+                else:
+                    # [upconv conv, deconv, deconv]: param_layers() names them conv0 / conv1 / conv2
+                    add([upconv(n)] + convs, False, stride * 2, None if norms is None else [None] + norms,
+                        upconv=True)
         add([conv(1, n_feat[-1], stride=1)], False, 1)               # back to 3 channels
         assert float(np.prod(self.spatsize_changes)) == 1, "Resolution doesn't return to the original value"
 

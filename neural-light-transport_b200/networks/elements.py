@@ -5,7 +5,7 @@ conv + norm + act triple of the reference is executed as ONE fused CUDA op
 (bias and activation live in the conv epilogue), so `norm`/`act`/`iden`
 return markers rather than callable layers.
 """
-from engine import ConvLayer, NormLayer  # noqa: F401
+from engine import ConvLayer, NormLayer, PoolLayer  # noqa: F401
 
 
 def conv(kernel_size, n_ch_out, stride=1):
@@ -17,9 +17,9 @@ def deconv(kernel_size, n_ch_out, stride=1):
 
 
 def upconv(n_ch_out):
-    raise NotImplementedError(
-        'upconv (bilinear x2 + conv2x2) is only reachable with pool != None, '
-        'which is outside this hot path (SURVEY.md 8a a5)')
+    """The conv half of `upconv` (UpSampling2D(2, 'bilinear') + Conv2D(n, 2, padding='same'), linear with bias).  The
+    upsampling is done by the Block that owns it (networks/convnet.py), once per distinct source of its input."""
+    return ConvLayer('conv', 2, 1, n_ch_out)
 
 
 def norm(type_):
@@ -45,7 +45,7 @@ def pool(type_):
     if type_ is None or type_.lower() == 'none':
         return None
     if type_ in ('max', 'avg'):
-        raise NotImplementedError('pool=%s is not on the accelerated path' % type_)
+        return PoolLayer(type_)
     raise NotImplementedError(type_)
 
 

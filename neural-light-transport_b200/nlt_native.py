@@ -94,6 +94,12 @@ _SIGS = {
     'nlt_instnorm_workspace_bytes': (C.c_int64, [C.c_int32] * 3),
     'nlt_instnorm_fwd': (C.c_int, [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_int, C.c_float] + [C.c_void_p] * 5),
     'nlt_instnorm_bwd': (C.c_int, [C.c_void_p] * 5 + [C.c_int32] * 3 + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 2),
+    'nlt_pool2x2_fwd': (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_int, C.c_void_p, C.c_void_p]),
+    'nlt_pool2x2_bwd': (C.c_int, [C.c_void_p] * 2 + [C.c_int32] * 4 + [C.c_int, C.c_float, C.c_void_p, C.c_int]
+                        + [C.c_void_p] * 2),
+    'nlt_upsample2x_bilinear_fwd': (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2),
+    'nlt_upsample2x_bilinear_bwd': (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_float, C.c_void_p, C.c_int]
+                                    + [C.c_void_p] * 2),
     'nlt_u8_to_f32': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'nlt_ksum_acc': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     'nlt_scale': (C.c_int, [C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),

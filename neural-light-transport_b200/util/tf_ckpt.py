@@ -18,6 +18,12 @@ Object-graph keys of the reference model (Keras tracking of `net_<network>_layer
   net/net_query_layer0/kernel/.ATTRIBUTES/VARIABLE_VALUE                          bare Conv2D (levels 0 and 13)
   net/net_query_layer3/layer_with_weights-1/bias/.ATTRIBUTES/VARIABLE_VALUE       j-th conv of a Sequential block
   .../kernel/.OPTIMIZER_SLOT/optimizer/{m,v,vhat}/.ATTRIBUTES/VARIABLE_VALUE      Adam slots; optimizer/iter/...
+  net/net_query_layer7/layer_with_weights-0/layer_with_weights-0/kernel/...       `pool != None`: the conv of the up
+                                                                                  block's nested upconv Sequential
+                                                                                  (conv0; the two deconvs are -1, -2)
+The nested upconv keys follow from Keras's `layer_with_weights-N` tracking of a Sequential inside a Sequential
+(nlt/networks/elements.py:42-48 inside convnet.py:66-75); like the rest of this reader they are unpinned, since no
+TF-written checkpoint of a pooling network exists offline.
 """
 import os
 import re
@@ -220,7 +226,7 @@ def load_nlt_state(prefix):
     'optimizer/iterations', 'step')."""
     raw = load_bundle(prefix)
     state = {}
-    pat = re.compile(r'^net/(net_\w+?_layer\d+)/(?:layer_with_weights-(\d+)/)?(kernel|bias)'
+    pat = re.compile(r'^net/(net_\w+?_layer\d+)/(?:layer_with_weights-(\d+)/)?(?:layer_with_weights-0/)?(kernel|bias)'
                      r'(?:/\.OPTIMIZER_SLOT/optimizer/(m|v|vhat))?' + re.escape(_SUFFIX) + '$')
     for key, arr in raw.items():
         m = pat.match(key)
@@ -340,9 +346,12 @@ def save_nlt_state(prefix, state):
             if not m:
                 continue
             slot, layer, j, leaf = m.groups()
-            # a bare Conv2D layer (one conv in the block) has no layer_with_weights level
+            # a bare Conv2D layer (one conv in the block) has no layer_with_weights level; a three-conv up block
+            # (pool != None) starts with the nested upconv Sequential, whose conv is its layer_with_weights-0
             single = not any(kk.endswith('%s/conv1/kernel' % layer) for kk in state)
-            path = 'net/%s/%s%s' % (layer, '' if single else 'layer_with_weights-%s/' % j, leaf)
+            nested = j == '0' and any(kk.endswith('%s/conv2/kernel' % layer) for kk in state)
+            path = 'net/%s/%s%s%s' % (layer, '' if single else 'layer_with_weights-%s/' % j,
+                                      'layer_with_weights-0/' if nested else '', leaf)
             if slot:
                 path += '/.OPTIMIZER_SLOT/optimizer/' + slot
             out[path + _SUFFIX] = np.asarray(v, dtype=np.float32)
