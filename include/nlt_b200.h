@@ -245,7 +245,9 @@ int nlt_amsgrad_step(float* p, const float* g, float* m, float* v, float* vhat,
  *            y = act(gamma * (x - mean_hw) * rsqrt(var_hw + eps) + beta), statistics per sample and channel
  *            (biased variance); _fwd also returns mean / rstd [N*C] for the backward pass; _bwd writes dx and
  *            (accumulate ? adds to : overwrites) dgamma / dbeta [C].  Deterministic (fixed-order reductions).
- *            workspace >= nlt_instnorm_workspace_bytes(). */
+ *            The variance is the centred second moment, taken per 1024-pixel chunk around the chunk's own mean and
+ *            merged in double (Chan), so rstd does not degrade as |mean| / std grows.
+ *            workspace >= nlt_instnorm_workspace_bytes() = (N * ceil(HW / 1024) * 3C + 2NC) floats; C <= 6144. */
 int nlt_pixelnorm_fwd(const float* x, int64_t pixels, int32_t C, int act, float* y, void* stream);
 int nlt_pixelnorm_bwd(const float* x, const float* dz, int64_t pixels, int32_t C, float* dx, void* stream);
 int64_t nlt_instnorm_workspace_bytes(int32_t N, int32_t HW, int32_t C);

@@ -84,28 +84,84 @@ pixelnorm_kernel(const float* __restrict__ x, const float* __restrict__ dz, floa
 // ---------------------------------------------------------------------------------------------
 constexpr int IN_CHUNK = 1024;                   // pixels per partial
 
-// partial[(n * nchunk + chunk) * 2C + {c, C + c}] = (sum a, sum b) over the chunk's pixels, where
-//   stats pass:    a = x,  b = x^2
-//   backward pass: a = dz, b = dz * xhat        (xhat from mean / rstd)
-template <bool BWD>
+// Thread layout of the two partial kernels.  C <= blockDim: thread = (row, channel), rows = blockDim / C pixel rows in
+// flight (loads coalesced along channels); C > blockDim: one row, every thread walks several channels.
+
+// Statistics pass: stat[(n * nchunk + chunk) * 3C + {c, C + c, 2C + c}] = (sum (x - a), sum (x - a)^2, a) over the
+// chunk's pixels, where a is the chunk's own mean as a first fp32 sweep finds it.  The second sweep re-reads the chunk
+// (1024 * C floats, cache resident at the channel counts of the large levels) around that shift, so neither sum
+// cancels however far a channel's mean lies from zero: E[x^2] - mean^2 on the raw values loses
+// (mean / std)^2 * 2^-24 of the variance.  sum (x - a) is the part of the chunk's sum the first sweep rounded away.
 __global__ void __launch_bounds__(256)
-instnorm_partial_kernel(const float* __restrict__ x, const float* __restrict__ dz, const float* __restrict__ mean,
-                        const float* __restrict__ rstd, int HW, int C, int nchunk, float* __restrict__ partial) {
+instnorm_stats_partial_kernel(const float* __restrict__ x, int HW, int C, int nchunk, float* __restrict__ stat) {
+  const int n = blockIdx.y, chunk = blockIdx.x;
+  const int p0 = chunk * IN_CHUNK, p1 = min(HW, p0 + IN_CHUNK);
+  const float inv_cnt = 1.f / (float)(p1 - p0);
+  extern __shared__ float sm[];                  // [rows][2C] partials of the thread rows
+  const int rows = (int)blockDim.x / C > 0 ? (int)blockDim.x / C : 1;
+  float* out = stat + ((size_t)n * nchunk + chunk) * 3 * C;
+  auto sweep = [&](int row, int c, float a, float& r, float& q) {
+    r = 0.f; q = 0.f;
+    for (int p = p0 + row; p < p1; p += rows) {
+      const float d = __ldg(x + ((size_t)n * HW + p) * C + c) - a;
+      r += d; q += d * d;
+    }
+  };
+  if (rows > 1) {                                // one (row, channel) per thread; the rows share the shift
+    const int row = threadIdx.x / C, c = threadIdx.x - row * C;
+    const bool live = row < rows;
+    float r, q;
+    if (live) { sweep(row, c, 0.f, r, q); sm[(size_t)row * 2 * C + c] = r; }
+    __syncthreads();
+    float a = 0.f;
+    if (live) {
+      for (int k = 0; k < rows; ++k) a += sm[(size_t)k * 2 * C + c];
+      a *= inv_cnt;
+    }
+    __syncthreads();
+    if (live) {
+      sweep(row, c, a, r, q);
+      sm[(size_t)row * 2 * C + c] = r;
+      sm[(size_t)row * 2 * C + C + c] = q;
+      if (row == 0) out[2 * C + c] = a;
+    }
+  } else {
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+      float r, q;
+      sweep(0, c, 0.f, r, q);
+      const float a = r * inv_cnt;
+      sweep(0, c, a, r, q);
+      sm[c] = r;
+      sm[C + c] = q;
+      out[2 * C + c] = a;
+    }
+  }
+  __syncthreads();
+  for (int j = threadIdx.x; j < 2 * C; j += blockDim.x) {
+    float s = 0.f;
+    for (int k = 0; k < rows; ++k) s += sm[(size_t)k * 2 * C + j];
+    out[j] = s;
+  }
+}
+
+// Backward pass: partial[(n * nchunk + chunk) * 2C + {c, C + c}] = (sum dz, sum dz * xhat) over the chunk's pixels
+// (xhat from mean / rstd)
+__global__ void __launch_bounds__(256)
+instnorm_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ dz, const float* __restrict__ mean,
+                            const float* __restrict__ rstd, int HW, int C, int nchunk, float* __restrict__ partial) {
   const int n = blockIdx.y, chunk = blockIdx.x;
   const int p0 = chunk * IN_CHUNK, p1 = min(HW, p0 + IN_CHUNK);
   extern __shared__ float sm[];                  // [rows][2C] partials of the thread rows
-  // C <= blockDim: thread = (row, channel), rows = blockDim / C pixel rows in flight (loads coalesced along channels);
-  // C > blockDim: one row, every thread walks several channels
   const int rows = (int)blockDim.x / C > 0 ? (int)blockDim.x / C : 1;
   for (int idx = threadIdx.x; idx < rows * C; idx += blockDim.x) {
     const int row = idx / C, c = idx - row * C;
     float a = 0.f, b = 0.f;
-    const float m = BWD ? mean[(size_t)n * C + c] : 0.f, rs = BWD ? rstd[(size_t)n * C + c] : 0.f;
+    const float m = mean[(size_t)n * C + c], rs = rstd[(size_t)n * C + c];
     for (int p = p0 + row; p < p1; p += rows) {
       const size_t i = ((size_t)n * HW + p) * C + c;
-      const float xv = __ldg(x + i);
-      if (!BWD) { a += xv; b += xv * xv; }
-      else { const float d = __ldg(dz + i); a += d; b += d * (xv - m) * rs; }
+      const float d = __ldg(dz + i);
+      a += d;
+      b += d * (__ldg(x + i) - m) * rs;
     }
     sm[(size_t)row * 2 * C + c] = a;
     sm[(size_t)row * 2 * C + C + c] = b;
@@ -118,22 +174,28 @@ instnorm_partial_kernel(const float* __restrict__ x, const float* __restrict__ d
   }
 }
 
-// mean / rstd per (n, c) from the partials (summed in double, fixed order)
-__global__ void instnorm_stats_kernel(const float* __restrict__ partial, int N, int HW, int C, int nchunk, float eps,
+// mean / rstd per (n, c): the chunks' (count, mean, centred second moment) merged in double, in chunk order, with
+// Chan's pairwise update
+__global__ void instnorm_stats_kernel(const float* __restrict__ stat, int N, int HW, int C, int nchunk, float eps,
                                       float* __restrict__ mean, float* __restrict__ rstd) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N * C) return;
   const int n = i / C, c = i - n * C;
-  double s = 0.0, s2 = 0.0;
+  double cnt = 0.0, m = 0.0, m2 = 0.0;
   for (int k = 0; k < nchunk; ++k) {
-    s += (double)partial[((size_t)n * nchunk + k) * 2 * C + c];
-    s2 += (double)partial[((size_t)n * nchunk + k) * 2 * C + C + c];
+    const float* s = stat + ((size_t)n * nchunk + k) * 3 * C;
+    const double nk = (double)(min(HW, (k + 1) * IN_CHUNK) - k * IN_CHUNK);
+    const double r = (double)s[c], q = (double)s[C + c];
+    const double mk = (double)s[2 * C + c] + r / nk;
+    double m2k = q - r * r / nk;
+    if (m2k < 0.0) m2k = 0.0;
+    const double d = mk - m, tot = cnt + nk;
+    m += d * nk / tot;
+    m2 += m2k + d * d * cnt * nk / tot;
+    cnt = tot;
   }
-  const double m = s / HW;
-  double var = s2 / HW - m * m;
-  if (var < 0.0) var = 0.0;
   mean[i] = (float)m;
-  rstd[i] = (float)(1.0 / sqrt(var + (double)eps));
+  rstd[i] = (float)(1.0 / sqrt(m2 / HW + (double)eps));
 }
 
 // per (n, c): sums of the backward partials -> (mean dz, mean dz*xhat); and the parameter gradients
@@ -221,19 +283,15 @@ int nlt_pixelnorm_bwd(const float* x, const float* dz, int64_t pixels, int32_t C
 int64_t nlt_instnorm_workspace_bytes(int32_t N, int32_t HW, int32_t C) {
   if (N <= 0 || HW <= 0 || C <= 0) return -1;
   const int64_t nchunk = (HW + IN_CHUNK - 1) / IN_CHUNK;
-  return ((int64_t)N * nchunk * 2 * C + 2 * (int64_t)N * C) * (int64_t)sizeof(float);
+  // forward: (sum, second moment, shift) per chunk and channel; backward: two sums per chunk and channel + mdz, mdzx
+  return ((int64_t)N * nchunk * 3 * C + 2 * (int64_t)N * C) * (int64_t)sizeof(float);
 }
 
-static int instnorm_partial_launch(bool bwd, const float* x, const float* dz, const float* mean, const float* rstd,
-                                   int N, int HW, int C, int nchunk, float* partial, cudaStream_t st) {
-  const int threads = 256;
-  const int rows = threads / C > 0 ? threads / C : 1;
-  const size_t smem = (size_t)rows * 2 * C * sizeof(float);
-  NLT_CHECK_ARG(smem <= 48 * 1024, "instance norm: too many channels (%d)", C);
-  dim3 grid(nchunk, N);
-  if (bwd) instnorm_partial_kernel<true><<<grid, threads, smem, st>>>(x, dz, mean, rstd, HW, C, nchunk, partial);
-  else instnorm_partial_kernel<false><<<grid, threads, smem, st>>>(x, nullptr, nullptr, nullptr, HW, C, nchunk, partial);
-  NLT_CUDA_LAUNCH_CHECK("instnorm_partial_kernel");
+// threads and shared memory of the two partial kernels (one [rows][2C] table)
+static int instnorm_partial_smem(int C, size_t* smem) {
+  const int rows = 256 / C > 0 ? 256 / C : 1;
+  *smem = (size_t)rows * 2 * C * sizeof(float);
+  NLT_CHECK_ARG(*smem <= 48 * 1024, "instance norm: too many channels (%d)", C);
   return NLT_OK;
 }
 
@@ -245,8 +303,11 @@ int nlt_instnorm_fwd(const float* x, const float* gamma, const float* beta, int3
   cudaStream_t st = (cudaStream_t)stream;
   const int nchunk = (HW + IN_CHUNK - 1) / IN_CHUNK;
   float* partial = (float*)workspace;
-  int rc = instnorm_partial_launch(false, x, nullptr, nullptr, nullptr, N, HW, C, nchunk, partial, st);
+  size_t smem;
+  int rc = instnorm_partial_smem(C, &smem);
   if (rc != NLT_OK) return rc;
+  instnorm_stats_partial_kernel<<<dim3(nchunk, N), 256, smem, st>>>(x, HW, C, nchunk, partial);
+  NLT_CUDA_LAUNCH_CHECK("instnorm_stats_partial_kernel");
   instnorm_stats_kernel<<<(N * C + 127) / 128, 128, 0, st>>>(partial, N, HW, C, nchunk, eps, mean, rstd);
   NLT_CUDA_LAUNCH_CHECK("instnorm_stats_kernel");
   const size_t total4 = (size_t)N * HW * C / 4;
@@ -266,8 +327,11 @@ int nlt_instnorm_bwd(const float* x, const float* dz, const float* gamma, const 
   float* partial = (float*)workspace;
   float* mdz = partial + (size_t)N * nchunk * 2 * C;
   float* mdzx = mdz + (size_t)N * C;
-  int rc = instnorm_partial_launch(true, x, dz, mean, rstd, N, HW, C, nchunk, partial, st);
+  size_t smem;
+  int rc = instnorm_partial_smem(C, &smem);
   if (rc != NLT_OK) return rc;
+  instnorm_bwd_partial_kernel<<<dim3(nchunk, N), 256, smem, st>>>(x, dz, mean, rstd, HW, C, nchunk, partial);
+  NLT_CUDA_LAUNCH_CHECK("instnorm_bwd_partial_kernel");
   instnorm_bwd_reduce_kernel<<<(C + 63) / 64, 64, 0, st>>>(partial, N, HW, C, nchunk, mdz, mdzx, dgamma, dbeta, accumulate);
   NLT_CUDA_LAUNCH_CHECK("instnorm_bwd_reduce_kernel");
   const size_t total4 = (size_t)N * HW * C / 4;
