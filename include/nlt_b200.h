@@ -223,8 +223,10 @@ int nlt_ssim_loss(const float* pred, const float* gt, int32_t B, int32_t H, int3
  *   r = (gt - pred) [* alpha]  ->  volume-preserving YUV  ->  `levels`-level CDF 9/7 analysis (reflecting
  *   boundaries)  ->  nll = sqrt((w/scale)^2 + 1) - 1 + log(scale) + log_z per coefficient
  *   loss[b] = mean_{h,w,c} nll ;  d_pred = d(sum_b loss[b] * loss_scale) / d(pred)
- * pred, gt: [B,H,W,3]; alpha: [B,H,W,1] or NULL; log_z = log Z(1) = log(2 e K_1(1)) = 1.18549523...;
- * levels <= ceil(log2(min(H, W))) (the reference uses 5); d_pred may be NULL; workspace >= _workspace_bytes(). */
+ * pred, gt: [B,H,W,3] with B <= 65535; alpha: [B,H,W,1] or NULL; log_z = log Z(1) = log(2 e K_1(1)) = 1.18549523...;
+ * levels <= ceil(log2(min(H, W))) (the reference uses 5); d_pred may be NULL (the loss is bit-identical either way).
+ * Deterministic: per-block partials summed per sample in a fixed order, in double.  workspace >= _workspace_bytes()
+ * (the wavelet planes plus B x (blocks per sample) doubles), 8-byte aligned, contents on entry irrelevant. */
 int64_t nlt_barron_loss_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t levels);
 int nlt_barron_loss(const float* pred, const float* gt, const float* alpha, int32_t B, int32_t H, int32_t W,
                     int32_t levels, float scale, float log_z, float loss_scale, float* loss, float* d_pred,

@@ -5,6 +5,7 @@
 //   residual (gt - pred)[* alpha]  ->  volume-preserving YUV (util.py:97-115)
 //   -> 5-level CDF 9/7 analysis, reflecting boundaries (wavelet.py:33-94, 170-218, 293-334)
 //   -> Charbonnier NLL per coefficient: sqrt((w/c)^2 + 1) - 1 + log c + log Z(1)   (general.py:96-122, distribution.py:181-222)
+//      (evaluated in a cancellation-free form, see charbonnier())
 //
 // One analysis step along an axis of length n:  out_lo[j] = sum_t lo[t] * x[R(2j     + t - 4)],  j < ceil(n/2)
 //                                               out_hi[j] = sum_t hi[t] * x[R(2j + 1 + t - 3)],  j < floor(n/2)
@@ -107,9 +108,12 @@ NLT_HD float adjoint_at(const float* g_lo, const float* g_hi, int n, int st_lo, 
 }
 
 // ---- robust loss at alpha = 1 ----
+// sqrt(z^2 + 1) - 1 written as z^2 / (sqrt(z^2 + 1) + 1): the same value without the cancellation that loses every
+// digit of the difference below |z| ~ 1e-2 (a converged model's coefficients sit there)
 NLT_HD float charbonnier(float w, float inv_scale) {
   const float z = w * inv_scale;
-  return sqrtf(z * z + 1.f) - 1.f;
+  const float z2 = z * z;
+  return z2 / (sqrtf(z2 + 1.f) + 1.f);
 }
 NLT_HD float charbonnier_grad(float w, float inv_scale) {
   const float z = w * inv_scale;

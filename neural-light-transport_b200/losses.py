@@ -118,7 +118,8 @@ class Barron():
     produces the per-sample losses and d(sum_b loss_b * grad_scale)/d(pred) (nlt_barron_loss).
 
     The arithmetic is checked on the CPU (tests/test_barron_core.py) and the kernels on hardware
-    (tests/test_gpu_barron.py) against the oracle that is pinned to the reference's own wavelet fixtures."""
+    (tests/test_gpu_barron.py, tests/test_gpu_barron_census.py) against the oracle that is pinned to the reference's
+    own wavelet fixtures.  The per-sample losses are deterministic."""
     LOG_Z_ALPHA1 = 1.1854952323491930      # log Z(1) = log(2 e K_1(1)); the reference's spline agrees to 1e-10
     SCALE = 0.01
     LEVELS = 5

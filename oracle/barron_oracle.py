@@ -68,7 +68,7 @@ def _filter_decimate(x, f, axis, shift):
     xp = x.index_select(dim, idx)
     xp = xp.narrow(dim, shift, xp.shape[dim] - shift)
     win = xp.unfold(dim, len(f), 2)                       # [..., n_out, ..., taps]
-    return (win * f.to(x.dtype)).sum(-1)
+    return (win * f.to(device=x.device, dtype=x.dtype)).sum(-1)
 
 
 def wavelet_construct(im, num_levels):
@@ -149,6 +149,32 @@ def image_nll(residual, log_z, scale=0.01, num_levels=5):
     flat = wavelet_flatten(wavelet_construct(stack, num_levels))
     mat = flat.reshape(n, c, h, w).permute(0, 2, 3, 1)
     return charbonnier(mat, scale) + math.log(scale) + log_z
+
+
+def image_nll_abs_grad(residual, scale=0.01, num_levels=5, grad_scale=1.0):
+    """Magnitude companion of d(grad_scale * sum image_nll(residual)) / d(residual): |M|^T |W|^T |g| in the residual's
+    [N, H, W, 3] layout, with g = grad_scale * d charbonnier / dw per wavelet coefficient, |W| the analysis run with
+    absolute filter taps and |M| the scaled YUV matrix with absolute entries.  Every product of the chain taken in
+    magnitude, so a computed gradient's rounding error is a few units of its precision times this, wherever the
+    signed sums cancel.  Multiply by |alpha| for an alpha-blended residual."""
+    n, h, w, c = residual.shape
+    stack = rgb_to_syuv(residual.detach()).permute(0, 3, 1, 2).reshape(n * c, h, w)
+    with torch.no_grad():
+        z = wavelet_flatten(wavelet_construct(stack, num_levels)) / scale
+    g = (grad_scale / scale) * (z / torch.sqrt(z * z + 1.0)).abs()
+    lo, hi = (f.abs() for f in cdf97_analysis_filters(residual.dtype))
+    x0 = torch.zeros_like(stack, requires_grad=True)
+    with torch.enable_grad():
+        im, pyr = x0, []
+        for _ in range(num_levels):         # wavelet_construct with |taps|
+            hr = _filter_decimate(im, hi, 0, 1)
+            lr = _filter_decimate(im, lo, 0, 0)
+            pyr.append((_filter_decimate(hr, hi, 1, 1), _filter_decimate(lr, hi, 1, 1), _filter_decimate(hr, lo, 1, 0)))
+            im = _filter_decimate(lr, lo, 1, 0)
+        pyr.append(im)
+        gx, = torch.autograd.grad(wavelet_flatten(tuple(pyr)), x0, g)
+    m = SYUV_SCALE * torch.tensor(_YUV_FROM_RGB, dtype=residual.dtype, device=residual.device).abs()
+    return gx.reshape(n, c, h, w).permute(0, 2, 3, 1) @ m.t()
 
 
 def barron_loss(gt, pred, log_z, keep_batch=False, weights=None):

@@ -90,7 +90,8 @@ extern "C" int barron_host(const float* pred, const float* gt, const float* alph
     acc[p / 3] += charbonnier(top.img[i], inv_scale);
     top.img[i] = gscale * charbonnier_grad(top.img[i], inv_scale);
   }
-  for (int b = 0; b < Bn; ++b) loss[b] = (float)(acc[b] * inv_count) + std::log(scale) + log_z;
+  const float constant = std::log(scale) + log_z;             // formed as the kernel forms it
+  for (int b = 0; b < Bn; ++b) loss[b] = (float)(acc[b] * (double)inv_count) + constant;
   if (!d_pred) return 0;
   for (int l = levels - 1; l >= 0; --l) {
     Level& c = lv[l];
