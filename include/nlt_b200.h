@@ -69,17 +69,14 @@ typedef struct nlt_gconv_desc {
 } nlt_gconv_desc;
 
 const char* nlt_version(void);
-/* process-wide switches: "tc" (1: wgmma 3xTF32 path where eligible [default], 0: fp32-FMA kernels only, 2: the wgmma
- * path for every shape it can run, ahead of the size heuristics and the stream kernels -- for A/B tests),
- * "tc_wgrad" (same for the weight-gradient kernel), "wgrad_rows" (1: row-run form of the warp-stream
- * weight-gradient kernel where float4 access allows it [default], 0: flat-pixel form), "dconv_wide" (1: the
- * pixel x 16-outputs stencil kernel for the 16-channel stencils, 0: the tiled implicit-GEMM kernel),
- * "dconv_wide32" (default 0 = off: the 32-output form of that kernel, validated but not faster;
- * 1 = one pixel per thread, 2 = two), "dconv_wide8" (default 1: the 8-output form, reached together
- * with "dconv_wide_first"), "dconv_wide_first" (routing, default 1: prefer the wide
- * stencil kernel over the quad-per-thread one for 16 / 8 outputs with K <= 32).
- * Environment defaults: NLT_DISABLE_TC=1, NLT_DISABLE_TC_WGRAD=1, NLT_DCONV_WIDE=0|1. */
+/* process-wide switches that select conv kernels: "tc", "tc_wgrad", "wgrad_rows", "tcs", "tc_rawhi", "tc_split_waves",
+ * "pwx", "pwmma", "tiny", "dconv_cw", "dconv_wide_first", "pf", "pf_s1", "pwd2s_first", "pf_ns", "pwx_ns", "wop",
+ * "dconv_wide", "dconv_wide32", "dconv_wide8".  The option table in csrc/nlt_gconv.cu gives each one's meaning,
+ * environment variable and default; an option takes its environment value or default when it is first read or set.
+ * "tc" = 2 is the wgmma path for every shape it can run (A/B tests).  Unknown names are an error. */
 int nlt_set_option(const char* name, int value);
+/* *value = the option's current value (what nlt_set_option stored, else its environment value or default) */
+int nlt_get_option(const char* name, int* value);
 const char* nlt_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process (diagnostic counter) */
 uint64_t nlt_launch_count(void);

@@ -23,6 +23,14 @@ void count_launch(const char* what);    // per-kernel launch counter behind nlt_
 // SMs of the current device: grid caps of the grid-stride and persistent kernels (cached per device)
 int sm_count();
 
+// process-wide switches, in the order of the option table in nlt_gconv.cu (name, environment variable, default)
+enum class Opt {
+  TC, TC_WGRAD, WGRAD_ROWS, TCS, TC_RAWHI, TC_SPLIT_WAVES, PWX, PWMMA, TINY, DCONV_CW, DCONV_WIDE_FIRST, PF, PF_S1,
+  PWD2S_FIRST, PF_NS, PWX_NS, WOP, DCONV_WIDE, DCONV_WIDE32, DCONV_WIDE8, COUNT
+};
+// the value of a switch: its environment variable or default on the first read, then whatever nlt_set_option stored
+int opt(Opt o);
+
 // two fp32 FMAs on a float pair (a * b + c per component, round-to-nearest)
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
   return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
@@ -170,20 +178,13 @@ bool pw_conv_applicable(const GConvK& k);
 bool pw_extra_applicable(const GConvK& k, const PwExtra& ex, const float* out, const float* mask_y);
 int launch_pw_conv(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act,
                    float* out, cudaStream_t st, const PwExtra* ex = nullptr);
-// wide stencil kernel (pixel x 16 outputs per thread); option "dconv_wide" / NLT_DCONV_WIDE
-#define NLT_DCONV_WIDE_DEFAULT 1
-extern int g_opt_dconv_wide;
-extern int g_opt_dconv_cw;       // constant-memory weight table form of the wide stencil kernel: 1 on (default)
-extern int g_opt_dconv_wide8;    // experimental 8-output form: 0 off (default), 1 on
-extern int g_opt_dconv_wide32;   // experimental 32-output form: 0 off (default), 1 one pixel / thread, 2 two pixels
+// wide stencil kernel (pixel x 16, 32 or 8 outputs per thread; options "dconv_wide", "dconv_wide32", "dconv_wide8")
 bool dconv_wide_applicable(const GConvK& k, const float* out, const float* mask_y);
 int launch_dconv_wide(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act,
                       float* out, cudaStream_t st);
 bool dconv_small_applicable(const GConvK& k);
 int launch_dconv_small(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act,
                        float* out, cudaStream_t st);
-// 1: row-run warp-stream wgrad where float4 access allows it (default), 0: flat-pixel kernel only
-extern int g_opt_wgrad_rows;
 bool wgrad_small_applicable(const GConvK& k);
 size_t wgrad_small_ws_floats(const GConvK& k);
 // fills w (nsplit, pix_per_split, ld, KG, GS) and *KD_pad for the reduce stage
@@ -194,12 +195,6 @@ size_t wgrad_tpp_ws_floats(const GConvK& k);
 int launch_wgrad_tpp(const GConvK& k, const float* G, float* ws, WgradK* w, size_t* KD_pad, cudaStream_t st);
 
 // wide pointwise conv into 16 channels (nlt_pwx.cu): level 0 of the 64-channel query stack
-extern int g_opt_pwx;
-extern int g_opt_pf_ns, g_opt_pwx_ns, g_opt_pf_s1;
-int pf_s1_level();
-extern int g_opt_tiny;
-extern int g_opt_tc_rawhi;
-extern int g_opt_wop;
 bool wopn_wgrad_applicable(const GConvK& k, const float* G);
 size_t wopn_wgrad_ws_floats(const GConvK& k);
 int launch_wopn_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size_t* KD_pad, cudaStream_t st);
@@ -226,8 +221,6 @@ bool pwd2s_applicable(const GConvK& k, const float* bias, int act, const float* 
 int launch_pwd2s(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
                  const PwExtra* ex);
 // the same op on the tensor cores (mma.sync 3xTF32), for every shape pwd2s_applicable accepts; option "pwmma"
-extern int g_opt_pwmma;
-bool pwmma_enabled();
 int launch_pwd2s_mma(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
                      const PwExtra* ex);
 
@@ -237,9 +230,6 @@ size_t pws_wgrad_ws_floats(const GConvK& k);
 int launch_pws_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size_t* KD_pad, cudaStream_t st);
 
 // wgmma tensor-core path (nlt_tc.cu)
-#define NLT_TCS_DEFAULT 1
-extern int g_opt_tcs;            // register form of the forward kernel (A operand split in registers, wgmma RS)
-extern int g_tc_force;           // option "tc" = 2: the tensor-core kernel for every shape it can run (A/B testing)
 extern unsigned long long g_tc_launches;
 bool tc_applicable(const GConvK& k);
 size_t tc_workspace_bytes(const GConvK& k);

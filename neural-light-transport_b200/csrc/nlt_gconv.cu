@@ -675,6 +675,205 @@ void count_launch(const char* what) {
     if (g_kl_name[i] == what || strcmp(g_kl_name[i], what) == 0) { ++g_kl_count[i]; return; }
   if (g_kl_n < 128) { g_kl_name[g_kl_n] = what; g_kl_count[g_kl_n++] = 1; }
 }
+
+// ---- process-wide switches ----------------------------------------------------------------------------------------
+// One row per option, in the order of enum Opt: the nlt_set_option name, the environment variable that gives its first
+// value (or none), how that variable is read (CHAR: `val` when its first character is `ch`, else the default; ATOI:
+// atoi), the default, and how a value v is stored, from the environment or from nlt_set_option (BOOL: v != 0; INT: v;
+// NS: 2 if v == 2, else 1; TC: 0 if v == 0, 2 if v == 2, else 1).
+enum class Parse { CHAR, ATOI };
+enum class Store { BOOL, INT, NS, TC };
+struct OptRow { const char *name, *env; Parse parse; char ch; int val, dflt; Store store; };
+static const OptRow kOpts[] = {
+    // 1: the wgmma 3xTF32 kernels where eligible; 0: the fp32-FMA kernels only; 2: the wgmma kernel for every shape it
+    // can run, ahead of its size heuristics and of the stream kernels (A/B tests)
+    {"tc", "NLT_DISABLE_TC", Parse::CHAR, '1', 0, 1, Store::TC},
+    {"tc_wgrad", "NLT_DISABLE_TC_WGRAD", Parse::CHAR, '1', 0, 1, Store::BOOL},   // the same for weight gradients
+    {"wgrad_rows", nullptr, Parse::CHAR, 0, 0, 1, Store::BOOL},   // row-run form of the warp-stream weight gradient
+    {"tcs", "NLT_TCS", Parse::ATOI, 0, 0, 1, Store::BOOL},        // wgmma forward: A operand split in registers
+    {"tc_rawhi", "NLT_TC_RAWHI", Parse::CHAR, '0', 0, 1, Store::BOOL},   // 3xTF32: hi truncated (1) or rounded (0)
+    {"tc_split_waves", "NLT_TC_SPLIT_WAVES", Parse::CHAR, '1', 1, 0, Store::BOOL},   // see tc_plan
+    {"pwx", "NLT_PWX", Parse::CHAR, '0', 0, 1, Store::BOOL},      // the kernels of nlt_pwx.cu (0: the general routes)
+    {"pwmma", "NLT_PWMMA", Parse::CHAR, '0', 0, 1, Store::BOOL},  // depth-to-space input gradient on mma.sync (tc on)
+    {"tiny", "NLT_TINY", Parse::CHAR, '0', 0, 1, Store::BOOL},    // the row-stream stencil kernel of nlt_tiny.cu
+    {"dconv_cw", "NLT_DCONV_CW", Parse::CHAR, '0', 0, 1, Store::BOOL},   // wide stencil weights in constant memory
+    // the wide stencil kernel ahead of the quad-per-thread one where both apply (16 / 8 outputs, K <= 32)
+    {"dconv_wide_first", "NLT_DCONV_WIDE_FIRST", Parse::CHAR, '0', 0, 1, Store::BOOL},
+    // staged-patch forward of the 2x2/s2 convs (nlt_pwx.cu).  H100, cfg4 step: the level-1/2 forward convs take
+    // 0.87 ms less on the general kernels
+    {"pf", "NLT_PF", Parse::CHAR, '1', 1, 0, Store::BOOL},
+    {"pf_s1", "NLT_PF_S1", Parse::CHAR, '1', 1, 0, Store::BOOL},   // with pf: also the stride-1 16 -> 16 stencils
+    // the pointwise depth-to-space kernel ahead of the wgmma kernel for the input gradients of 2x2/s2 convs from
+    // 64-channel sources.  H100, cfg4 step: the wgmma kernel is faster there (level-3 input gradients 0.64 ms less)
+    {"pwd2s_first", "NLT_PWD2S_FIRST", Parse::CHAR, '1', 1, 0, Store::BOOL},
+    {"pf_ns", "NLT_PF_NS", Parse::CHAR, '2', 2, 1, Store::NS},     // threads per pixel of the staged-patch forward
+    {"pwx_ns", "NLT_PWX_NS", Parse::CHAR, '2', 2, 1, Store::NS},   // ... and of the pointwise forward
+    // outer-product weight gradients (nlt_wop.cu): 0 off; 1 the 4 -> 4 and 8 -> 8 stencils and the final 1x1 conv; 2
+    // also the 16 -> 16 stencils and the up-convs, where they are slower than the staged-patch / wgmma kernels
+    // (16 warps/SM at 128 registers cannot hide the load latency)
+    {"wop", "NLT_WOP", Parse::ATOI, 0, 0, 1, Store::INT},
+    {"dconv_wide", "NLT_DCONV_WIDE", Parse::ATOI, 0, 0, 1, Store::BOOL},   // wide stencil kernel, 16 outputs
+    {"dconv_wide32", "NLT_DCONV_WIDE32", Parse::ATOI, 0, 0, 0, Store::INT},   // 32 outputs: 1 / 2 pixels per thread
+    {"dconv_wide8", "NLT_DCONV_WIDE8", Parse::ATOI, 0, 0, 1, Store::INT},     // 8 outputs when > 0
+};
+static_assert(sizeof(kOpts) / sizeof(kOpts[0]) == (size_t)Opt::COUNT, "one row per option");
+static int opt_value[(int)Opt::COUNT];
+static bool opt_taken[(int)Opt::COUNT];   // the value has been read from the environment or set
+
+static int opt_index(const char* name) {
+  for (int i = 0; i < (int)Opt::COUNT; ++i)
+    if (strcmp(kOpts[i].name, name) == 0) return i;
+  return -1;
+}
+
+static void set_opt(int i, int v) {
+  const Store s = kOpts[i].store;
+  opt_value[i] = s == Store::INT ? v : s == Store::BOOL ? v != 0
+               : s == Store::NS ? (v == 2 ? 2 : 1) : (v == 0 ? 0 : (v == 2 ? 2 : 1));
+  opt_taken[i] = true;
+}
+
+int opt(Opt o) {
+  const int i = (int)o;
+  if (!opt_taken[i]) {
+    const OptRow& r = kOpts[i];
+    const char* e = r.env != nullptr ? getenv(r.env) : nullptr;
+    set_opt(i, e == nullptr ? r.dflt : r.parse == Parse::ATOI ? atoi(e) : (e[0] == r.ch ? r.val : r.dflt));
+  }
+  return opt_value[i];
+}
+
+// ---- kernel routes ------------------------------------------------------------------------------------------------
+// The route functions apply every option that selects a kernel; the *_applicable / *_plan predicates test shape and
+// alignment only.  Options that pick a variant inside one kernel's launch are read where that launch is configured.
+enum class Route { NONE, TC, PF, TINY, PWX, PWX_D2S, PWD2S, PWD2S_MMA, PW, DCONV_WIDE, DCONV_SMALL, TILED };
+
+// depth-to-space input gradient: the tensor-core form unless tc = 0 or pwmma = 0 (then the fp32 FMA kernel)
+static Route pwd2s_route() { return opt(Opt::TC) && opt(Opt::PWMMA) ? Route::PWD2S_MMA : Route::PWD2S; }
+
+// Kernel of a forward or input-gradient op that runs as one launch, in order of preference; Route::NONE: each phase
+// takes its phase_route.  The wgmma kernel needs its workspace within `ws_bytes` (< 0: no workspace, so the op stays
+// on the fp32 kernels).
+static Route fwd_route(const GConvK* ph, int np, const float* bias, int act, float beta, const float* mask_y,
+                       const float* out, int64_t ws_bytes) {
+  if (np != 1 || ph[0].M == 0) return Route::NONE;
+  const GConvK& k = ph[0];
+  auto tc = [&] {
+    return opt(Opt::TC) && tc_applicable(k) && ws_bytes >= 0 && (int64_t)tc_workspace_bytes(k) <= ws_bytes;
+  };
+  if (opt(Opt::TC) == 2 && tc()) return Route::TC;
+  // staged-patch forward; its stride-1 form only with pf_s1
+  const bool pf = opt(Opt::PF) && opt(Opt::PWX) && pf_fwd_applicable(k, mask_y, out) && (k.ay.it != 1 || opt(Opt::PF_S1));
+  // few-channel stride-1 stencils (4/8/16 -> same): the row-stream kernel of nlt_tiny.cu, ahead of the tensor path
+  // (16 -> 16 at 512^2 is a 130 B/pixel stream: the wgmma pipeline's fixed costs exceed its 0.5 kFMA/pixel)
+  if (pf && k.ay.it == 1) return Route::PF;
+  if (opt(Opt::TINY) && tiny_stencil_applicable(k, out, mask_y)) return Route::TINY;
+  // 2x2 / stride-2 convs of levels 1-2 (K = 64 / 128 into 16 / 32 channels)
+  if (pf) return Route::PF;
+  // up-convs into 4 / 8 channels: depth-to-space pointwise kernel with constant-bank weights (nlt_pwx.cu)
+  if (opt(Opt::PWX) && pwx_d2s_fwd_applicable(k, beta, mask_y, out)) return Route::PWX_D2S;
+  // input gradients of the 2x2 / stride-2 convs into 32-channel sources with K = 64 (level 3)
+  if (opt(Opt::PWD2S_FIRST) && opt(Opt::PWX) && k.d2s && k.nseg == 1 && k.seg[0].C == 64 &&
+      pwd2s_applicable(k, bias, act, out, mask_y, nullptr))
+    return Route::PWD2S;
+  return tc() ? Route::TC : Route::NONE;
+}
+
+// kernel of one phase of a forward or input-gradient op
+static Route phase_route(const GConvK& k, const float* bias, int act, float beta, const float* mask_y,
+                         const float* out) {
+  if (opt(Opt::PWX) && pwx_fwd_applicable(k, beta, mask_y, out)) return Route::PWX;
+  if (opt(Opt::PWX) && pwd2s_applicable(k, bias, act, out, mask_y, nullptr)) return pwd2s_route();
+  if (pw_conv_applicable(k)) return Route::PW;
+  if (opt(Opt::TINY) && tiny_stencil_applicable(k, out, mask_y)) return Route::TINY;
+  // wide stencil kernel: options dconv_wide / dconv_wide32 / dconv_wide8 for its 16- / 32- / 8-output forms
+  const bool wide = dconv_wide_applicable(k, out, mask_y) &&
+                    opt(k.Cout == 16 ? Opt::DCONV_WIDE : (k.Cout == 32 ? Opt::DCONV_WIDE32 : Opt::DCONV_WIDE8)) > 0;
+  if (dconv_small_applicable(k)) return wide && opt(Opt::DCONV_WIDE_FIRST) ? Route::DCONV_WIDE : Route::DCONV_SMALL;
+  return wide ? Route::DCONV_WIDE : Route::TILED;
+}
+
+// single-phase pointwise op with a fused pointwise term: the depth-to-space kernel or the pointwise kernel
+static Route fused_route(const GConvK& k, const PwExtra& ex, const float* bias, int act, const float* mask_y,
+                         const float* out) {
+  if (k.M == 0) return Route::NONE;
+  if (opt(Opt::PWX) && pwd2s_applicable(k, bias, act, out, mask_y, &ex)) return pwd2s_route();
+  return pw_extra_applicable(k, ex, out, mask_y) ? Route::PW : Route::NONE;
+}
+
+static int launch_route(Route r, const GConvK& k, const float* bias, int act, float beta, const float* mask_y,
+                        int mask_act, float* out, const PwExtra* ex, void* ws, int64_t ws_bytes, bool prepacked,
+                        cudaStream_t st) {
+  switch (r) {
+    case Route::TC: return launch_tc(k, bias, act, beta, mask_y, mask_act, out, ws, (size_t)ws_bytes, st, prepacked);
+    case Route::PF: return launch_pf_fwd(k, bias, act, beta, mask_y, mask_act, out, st);
+    case Route::TINY: return launch_tiny_stencil(k, bias, act, beta, mask_y, mask_act, out, st);
+    case Route::PWX: return launch_pwx_fwd(k, bias, act, out, st);
+    case Route::PWX_D2S: return launch_pwx_d2s_fwd(k, bias, act, out, st);
+    case Route::PWD2S: return launch_pwd2s(k, beta, mask_y, mask_act, out, st, ex);
+    case Route::PWD2S_MMA: return launch_pwd2s_mma(k, beta, mask_y, mask_act, out, st, ex);
+    case Route::PW: return launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, st, ex);
+    case Route::DCONV_WIDE: return launch_dconv_wide(k, bias, act, beta, mask_y, mask_act, out, st);
+    case Route::DCONV_SMALL: return launch_dconv_small(k, bias, act, beta, mask_y, mask_act, out, st);
+    case Route::TILED:
+      if (k.Cout > 32) return launch_fwd<128, 64, 8, 8>(k, bias, act, beta, mask_y, mask_act, out, st);
+      if (k.Cout > 16) return launch_fwd<128, 32, 8, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
+      if (k.Cout > 8) return launch_fwd<256, 16, 8, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
+      if (k.Cout > 4) return launch_fwd<256, 8, 4, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
+      return launch_fwd<256, 4, 2, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
+    case Route::NONE: break;
+  }
+  return set_err(NLT_ERR_INVALID, "no kernel route");
+}
+
+enum class WgradRoute { PWX, WOP, WOPN, PWS, TC, TPP, SMALL, TILED };
+
+// outer-product weight gradient: option wop = 1 for shapes into <= 8 channels outside depth-to-space, 2 for all
+static bool wop_on(const GConvK& k) { return opt(Opt::WOP) >= 2 || (opt(Opt::WOP) == 1 && !k.d2s && k.Cout <= 8); }
+
+// tensor-core weight gradient for this phase?  The row-run warp-stream kernel takes the shapes it applies to
+// (<= 16 gradient channels, K-depth <= 160: the level-1 32 -> 16 down-conv), the wgmma kernel everything else.
+static bool use_tc_wgrad(const GConvK& k) {
+  return opt(Opt::TC) && opt(Opt::TC_WGRAD) && tc_wgrad_applicable(k) && !wgrad_small_applicable(k);
+}
+
+// a k == stride transposed conv keeps its one-pass depth-to-space form when a kernel takes it (the warp-stream
+// kernel for narrow tiles, the wgmma kernel from K_d = 128 up); otherwise it runs as s*s phases
+static bool wgrad_keeps_d2s(const GConvK& k, const float* G) {
+  return (opt(Opt::PWX) && pwx_wgrad_applicable(k, G)) || (wop_on(k) && wop_wgrad_applicable(k, G)) ||
+         wgrad_small_applicable(k) || use_tc_wgrad(k);
+}
+
+static size_t wgrad_ws_floats(WgradRoute r, const GConvK& k) {
+  switch (r) {
+    case WgradRoute::PWX: return pwx_wgrad_ws_floats(k);
+    case WgradRoute::WOP: return wop_wgrad_ws_floats(k);
+    case WgradRoute::WOPN: return wopn_wgrad_ws_floats(k);
+    case WgradRoute::PWS: return pws_wgrad_ws_floats(k);
+    case WgradRoute::TC: return tc_wgrad_ws_floats(k);
+    case WgradRoute::TPP: return wgrad_tpp_ws_floats(k);
+    case WgradRoute::SMALL: return wgrad_small_ws_floats(k);
+    case WgradRoute::TILED: break;
+  }
+  return plan_wgrad(k).ws_floats;
+}
+
+// Weight-gradient kernel of one phase, in order of preference.  The first four give way to the next route when their
+// workspace exceeds `ws_bytes`; the workspace query asks with G = nullptr and no limit.
+static WgradRoute wgrad_route(const GConvK& k, const float* G, int64_t ws_bytes) {
+  auto fits = [&](WgradRoute r) { return (int64_t)(wgrad_ws_floats(r, k) * sizeof(float)) <= ws_bytes; };
+  if (opt(Opt::PWX) && pwx_wgrad_applicable(k, G) && fits(WgradRoute::PWX)) return WgradRoute::PWX;
+  // few-channel layers at (near) full resolution: register-tile outer products, one warp per unit kind (nlt_wop.cu)
+  if (wop_on(k) && wop_wgrad_applicable(k, G) && fits(WgradRoute::WOP)) return WgradRoute::WOP;
+  // final 1x1 conv into <= 4 channels: coalesced (pixel, channel quad) lanes (nlt_wop.cu)
+  if (opt(Opt::WOP) > 0 && wopn_wgrad_applicable(k, G) && fits(WgradRoute::WOPN)) return WgradRoute::WOPN;
+  if (opt(Opt::PWX) && pws_wgrad_applicable(k, G) && fits(WgradRoute::PWS)) return WgradRoute::PWS;
+  if (use_tc_wgrad(k)) return WgradRoute::TC;
+  if (wgrad_tpp_applicable(k)) return WgradRoute::TPP;
+  if (wgrad_small_applicable(k)) return WgradRoute::SMALL;
+  return WgradRoute::TILED;
+}
+
 }  // namespace nlt
 
 extern "C" {
@@ -692,94 +891,33 @@ uint64_t nlt_kernel_launch_count(const char* name) {
 }
 uint64_t nlt_tc_launch_count(void) { return __atomic_load_n(&nlt::g_tc_launches, __ATOMIC_RELAXED); }
 
-static int g_opt_tc = -1, g_opt_tc_wgrad = -1;   // -1: take the environment default
-// option "pwd2s_first" / NLT_PWD2S_FIRST (default 0): the pointwise depth-to-space kernel ahead of the wgmma kernel for
-// the input gradients of 2x2/s2 convs from 64-channel sources.  H100, cfg4 step: the wgmma kernel is faster there
-// (level-3 input gradients 0.64 ms less per step)
-static int g_opt_pwd2s_first = -1;
-static bool pwd2s_first() {
-  if (g_opt_pwd2s_first < 0) { const char* e = getenv("NLT_PWD2S_FIRST"); g_opt_pwd2s_first = (e && e[0] == '1') ? 1 : 0; }
-  return g_opt_pwd2s_first == 1;
-}
-// option "pf" / NLT_PF (default 0): staged-patch forward of nlt_pwx.cu.  H100, cfg4 step: the level-1/2 forward convs
-// take 0.87 ms less on the general kernels
-static int g_opt_pf = -1;
-static bool pf_enabled() {
-  if (g_opt_pf < 0) { const char* e = getenv("NLT_PF"); g_opt_pf = (e && e[0] == '1') ? 1 : 0; }
-  return g_opt_pf == 1;
-}
-static int g_opt_dconv_wide_first = -1;          // routing switch (NLT_DCONV_WIDE_FIRST, default 1), see nlt_gconv_fwd_ws
-static bool dconv_wide_first() {
-  if (g_opt_dconv_wide_first < 0) { const char* e = getenv("NLT_DCONV_WIDE_FIRST"); g_opt_dconv_wide_first = (e && e[0] == '0') ? 0 : 1; }
-  return g_opt_dconv_wide_first == 1;
-}
-static bool tc_enabled() {
-  if (g_opt_tc < 0) { const char* e = getenv("NLT_DISABLE_TC"); g_opt_tc = (e && e[0] == '1') ? 0 : 1; }
-  return g_opt_tc == 1;
-}
-
-// tensor-core weight gradient for this phase?  The row-run warp-stream kernel takes the shapes it applies to
-// (<= 16 gradient channels, K-depth <= 160: the level-1 32 -> 16 down-conv), the wgmma kernel everything else.
-static bool tc_wgrad_enabled();
-static bool use_tc_wgrad(const GConvK& k) {
-  return tc_wgrad_enabled() && tc_wgrad_applicable(k) && !wgrad_small_applicable(k);
-}
-
-static bool tc_wgrad_enabled() {
-  if (g_opt_tc_wgrad < 0) { const char* e = getenv("NLT_DISABLE_TC_WGRAD"); g_opt_tc_wgrad = (e && e[0] == '1') ? 0 : 1; }
-  return tc_enabled() && g_opt_tc_wgrad == 1;
-}
-
-// depth-to-space input gradient: the tensor-core form unless tc = 0 or pwmma = 0 (then the fp32 FMA kernel)
-static int launch_pwd2s_route(const GConvK& k, float beta, const float* mask_y, int mask_act, float* out, cudaStream_t st,
-                              const PwExtra* ex) {
-  if (tc_enabled() && pwmma_enabled()) return launch_pwd2s_mma(k, beta, mask_y, mask_act, out, st, ex);
-  return launch_pwd2s(k, beta, mask_y, mask_act, out, st, ex);
-}
-
 int nlt_set_option(const char* name, int value) {
   NLT_CHECK_ARG(name != nullptr, "null option name");
-  if (strcmp(name, "tc") == 0) { g_opt_tc = value ? 1 : 0; nlt::g_tc_force = value == 2; return NLT_OK; }
-  if (strcmp(name, "tc_wgrad") == 0) { g_opt_tc_wgrad = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "wgrad_rows") == 0) { nlt::g_opt_wgrad_rows = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "tcs") == 0) { nlt::g_opt_tcs = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "pwx") == 0) { nlt::g_opt_pwx = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "pwmma") == 0) { nlt::g_opt_pwmma = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "tc_rawhi") == 0) { nlt::g_opt_tc_rawhi = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "pwd2s_first") == 0) { g_opt_pwd2s_first = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "pf_s1") == 0) { nlt::g_opt_pf_s1 = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "pf_ns") == 0) { nlt::g_opt_pf_ns = value == 2 ? 2 : 1; return NLT_OK; }
-  if (strcmp(name, "pwx_ns") == 0) { nlt::g_opt_pwx_ns = value == 2 ? 2 : 1; return NLT_OK; }
-  if (strcmp(name, "pf") == 0) { g_opt_pf = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "wop") == 0) { nlt::g_opt_wop = value; return NLT_OK; }
-  if (strcmp(name, "tiny") == 0) { nlt::g_opt_tiny = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "dconv_cw") == 0) { nlt::g_opt_dconv_cw = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "dconv_wide") == 0) { nlt::g_opt_dconv_wide = value ? 1 : 0; return NLT_OK; }
-  if (strcmp(name, "dconv_wide32") == 0) { nlt::g_opt_dconv_wide32 = value; return NLT_OK; }
-  if (strcmp(name, "dconv_wide8") == 0) { nlt::g_opt_dconv_wide8 = value; return NLT_OK; }
-  if (strcmp(name, "dconv_wide_first") == 0) { g_opt_dconv_wide_first = value ? 1 : 0; return NLT_OK; }
-  return set_err(NLT_ERR_INVALID, "unknown option '%s'", name);
+  const int i = opt_index(name);
+  if (i < 0) return set_err(NLT_ERR_INVALID, "unknown option '%s'", name);
+  set_opt(i, value);
+  return NLT_OK;
+}
+
+int nlt_get_option(const char* name, int* value) {
+  NLT_CHECK_ARG(name != nullptr && value != nullptr, "null argument");
+  const int i = opt_index(name);
+  if (i < 0) return set_err(NLT_ERR_INVALID, "unknown option '%s'", name);
+  *value = opt((Opt)i);
+  return NLT_OK;
 }
 
 int64_t nlt_gconv_fwd_workspace_bytes(const nlt_gconv_desc* d) {
   GConvK ph[16];
   int np = 0;
   if (build_phases(d, ph, &np, /*allow_d2s=*/true) != NLT_OK) return -1;
-  if (np == 1 && tc_enabled() && tc_applicable(ph[0])) return (int64_t)tc_workspace_bytes(ph[0]);
+  if (np == 1 && opt(Opt::TC) && tc_applicable(ph[0])) return (int64_t)tc_workspace_bytes(ph[0]);
   return 0;
 }
 
-// does the forward of `d` run on the wgmma kernel (which reads packed hi / lo weight planes)?  Mirrors the routing
-// order of gconv_fwd_impl below.
+// does the forward of `d` run on the wgmma kernel (which reads packed hi / lo weight planes)?
 static bool fwd_takes_tc(const GConvK* ph, int np, float beta, const float* mask_y, const float* out) {
-  if (np != 1 || ph[0].M == 0) return false;
-  if (g_tc_force) return tc_enabled() && tc_applicable(ph[0]);
-  if (pf_enabled() && pf_fwd_applicable(ph[0], mask_y, out)) return false;
-  if (tiny_stencil_applicable(ph[0], out, mask_y)) return false;
-  if (pwx_d2s_fwd_applicable(ph[0], beta, mask_y, out)) return false;
-  if (pwd2s_first() && ph[0].d2s && ph[0].nseg == 1 && ph[0].seg[0].C == 64 &&
-      pwd2s_applicable(ph[0], nullptr, 0, out, mask_y, nullptr)) return false;
-  return tc_enabled() && tc_applicable(ph[0]);
+  return fwd_route(ph, np, nullptr, 0, beta, mask_y, out, INT64_MAX) == Route::TC;
 }
 
 int64_t nlt_gconv_fwd_pack_bytes(const nlt_gconv_desc* d, float beta, int has_mask) {
@@ -796,21 +934,8 @@ int nlt_gconv_pack_weights(const nlt_gconv_desc* d, void* packed, int64_t packed
   int np = 0;
   int rc = build_phases(d, ph, &np, /*allow_d2s=*/true);
   if (rc != NLT_OK) return rc;
-  NLT_CHECK_ARG(np == 1 && tc_enabled() && tc_applicable(ph[0]), "this op does not run on the tensor-core kernel");
+  NLT_CHECK_ARG(np == 1 && opt(Opt::TC) && tc_applicable(ph[0]), "this op does not run on the tensor-core kernel");
   return tc_pack(ph[0], packed, (size_t)packed_bytes, (cudaStream_t)stream);
-}
-
-static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
-                          int mask_act, float* out, void* workspace, int64_t workspace_bytes, void* stream, bool prepacked);
-
-int nlt_gconv_fwd_ws(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
-                     int mask_act, float* out, void* workspace, int64_t workspace_bytes, void* stream) {
-  return gconv_fwd_impl(d, bias, act, beta, mask_y, mask_act, out, workspace, workspace_bytes, stream, false);
-}
-
-int nlt_gconv_fwd_packed(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
-                         int mask_act, float* out, const void* packed, int64_t packed_bytes, void* stream) {
-  return gconv_fwd_impl(d, bias, act, beta, mask_y, mask_act, out, const_cast<void*>(packed), packed_bytes, stream, true);
 }
 
 static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
@@ -823,53 +948,34 @@ static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, f
   NLT_CHECK_ARG(act >= 0 && act <= 3 && mask_act >= 0 && mask_act <= 3, "bad activation code");
   NLT_CHECK_ARG(beta == 0.f || beta == 1.f, "beta must be 0 or 1");
   cudaStream_t st = (cudaStream_t)stream;
-  if (np == 1 && g_tc_force && workspace != nullptr && tc_enabled() && ph[0].M > 0 && tc_applicable(ph[0]) &&
-      (int64_t)tc_workspace_bytes(ph[0]) <= workspace_bytes)
-    return launch_tc(ph[0], bias, act, beta, mask_y, mask_act, out, workspace, (size_t)workspace_bytes, st, prepacked);
-  // few-channel stride-1 stencils (4/8/16 -> same): the row-stream kernel of nlt_tiny.cu, ahead of the tensor path
-  // (16 -> 16 at 512^2 is a 130 B/pixel stream: the wgmma pipeline's fixed costs exceed its 0.5 kFMA/pixel)
-  if (np == 1 && ph[0].M > 0 && pf_enabled() && pf_s1_level() > 0 && ph[0].ay.it == 1 && pf_fwd_applicable(ph[0], mask_y, out))
-    return launch_pf_fwd(ph[0], bias, act, beta, mask_y, mask_act, out, st);
-  if (np == 1 && ph[0].M > 0 && tiny_stencil_applicable(ph[0], out, mask_y))
-    return launch_tiny_stencil(ph[0], bias, act, beta, mask_y, mask_act, out, st);
-  // 2x2 / stride-2 convs of levels 1-2 (K = 64 / 128 into 16 / 32 channels): staged-patch forward (nlt_pwx.cu, option "pf")
-  if (np == 1 && pf_enabled() && pf_fwd_applicable(ph[0], mask_y, out))
-    return launch_pf_fwd(ph[0], bias, act, beta, mask_y, mask_act, out, st);
-  // up-convs into 4 / 8 channels: depth-to-space pointwise kernel with constant-bank weights (nlt_pwx.cu)
-  if (np == 1 && pwx_d2s_fwd_applicable(ph[0], beta, mask_y, out)) return launch_pwx_d2s_fwd(ph[0], bias, act, out, st);
-  // input gradients of the 2x2 / stride-2 convs into 32-channel sources with K = 64 (level 3): depth-to-space
-  // kernel ahead of the tensor path (option "pwd2s_first" / NLT_PWD2S_FIRST)
-  if (!prepacked && np == 1 && ph[0].M > 0 && pwd2s_first() && ph[0].d2s && ph[0].nseg == 1 && ph[0].seg[0].C == 64 &&
-      pwd2s_applicable(ph[0], bias, act, out, mask_y, nullptr))
-    return launch_pwd2s(ph[0], beta, mask_y, mask_act, out, st, nullptr);
+  // packed weights are only for an op that nlt_gconv_fwd_pack_bytes puts on the wgmma kernel: route it as that query
+  // does (no bias)
+  const Route r = fwd_route(ph, np, prepacked ? nullptr : bias, prepacked ? 0 : act, beta, mask_y, out,
+                            workspace != nullptr ? workspace_bytes : -1);
   if (prepacked)
-    NLT_CHECK_ARG(fwd_takes_tc(ph, np, beta, mask_y, out) && workspace != nullptr &&
-                  (int64_t)tc_workspace_bytes(ph[0]) <= workspace_bytes,
+    NLT_CHECK_ARG(r != Route::NONE && r != Route::PWD2S,
                   "nlt_gconv_fwd_packed: this op does not run on the tensor-core kernel (nlt_gconv_fwd_pack_bytes == 0)");
-  if (np == 1 && workspace != nullptr && tc_enabled() && ph[0].M > 0 && tc_applicable(ph[0]) &&
-      (int64_t)tc_workspace_bytes(ph[0]) <= workspace_bytes)
-    return launch_tc(ph[0], bias, act, beta, mask_y, mask_act, out, workspace, (size_t)workspace_bytes, st, prepacked);
+  if (r != Route::NONE)
+    return launch_route(r, ph[0], bias, act, beta, mask_y, mask_act, out, nullptr, workspace, workspace_bytes, prepacked,
+                        st);
   for (int i = 0; i < np; ++i) {
     const GConvK& k = ph[i];
     if (k.M == 0) continue;
-    if (pwx_fwd_applicable(k, beta, mask_y, out)) rc = launch_pwx_fwd(k, bias, act, out, st);
-    else if (pwd2s_applicable(k, bias, act, out, mask_y, nullptr)) rc = launch_pwd2s_route(k, beta, mask_y, mask_act, out, st, nullptr);
-    else if (pw_conv_applicable(k)) rc = launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (tiny_stencil_applicable(k, out, mask_y)) rc = launch_tiny_stencil(k, bias, act, beta, mask_y, mask_act, out, st);
-    // option "dconv_wide_first" (default on): prefer the wide stencil kernel over the quad-per-thread one where both apply
-    // (16 / 8 outputs, K <= 32: the up-conv input gradients of levels 11-12)
-    else if (dconv_wide_first() && dconv_small_applicable(k) && dconv_wide_applicable(k, out, mask_y))
-      rc = launch_dconv_wide(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (dconv_small_applicable(k)) rc = launch_dconv_small(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (dconv_wide_applicable(k, out, mask_y)) rc = launch_dconv_wide(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (k.Cout > 32) rc = launch_fwd<128, 64, 8, 8>(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (k.Cout > 16) rc = launch_fwd<128, 32, 8, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (k.Cout > 8) rc = launch_fwd<256, 16, 8, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
-    else if (k.Cout > 4) rc = launch_fwd<256, 8, 4, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
-    else rc = launch_fwd<256, 4, 2, 4>(k, bias, act, beta, mask_y, mask_act, out, st);
+    rc = launch_route(phase_route(k, bias, act, beta, mask_y, out), k, bias, act, beta, mask_y, mask_act, out, nullptr,
+                      nullptr, 0, false, st);
     if (rc != NLT_OK) return rc;
   }
   return NLT_OK;
+}
+
+int nlt_gconv_fwd_ws(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
+                     int mask_act, float* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  return gconv_fwd_impl(d, bias, act, beta, mask_y, mask_act, out, workspace, workspace_bytes, stream, false);
+}
+
+int nlt_gconv_fwd_packed(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
+                         int mask_act, float* out, const void* packed, int64_t packed_bytes, void* stream) {
+  return gconv_fwd_impl(d, bias, act, beta, mask_y, mask_act, out, const_cast<void*>(packed), packed_bytes, stream, true);
 }
 
 static int pw_term_phase(const nlt_gconv_desc* d, const nlt_pw_term* term, GConvK* k, PwExtra* ex) {
@@ -889,7 +995,7 @@ int nlt_gconv_fwd_fused_supported(const nlt_gconv_desc* d, const nlt_pw_term* te
   GConvK k;
   PwExtra ex;
   if (pw_term_phase(d, term, &k, &ex) != NLT_OK) return 0;
-  return (k.M > 0 && (pwd2s_applicable(k, nullptr, 0, out, mask_y, &ex) || pw_extra_applicable(k, ex, out, mask_y))) ? 1 : 0;
+  return fused_route(k, ex, nullptr, 0, mask_y, out) != Route::NONE ? 1 : 0;
 }
 
 int nlt_gconv_fwd_fused(const nlt_gconv_desc* d, const nlt_pw_term* term, const float* bias, int act, float beta,
@@ -902,11 +1008,9 @@ int nlt_gconv_fwd_fused(const nlt_gconv_desc* d, const nlt_pw_term* term, const 
   NLT_CHECK_ARG(out != nullptr, "null output");
   NLT_CHECK_ARG(act >= 0 && act <= 3 && mask_act >= 0 && mask_act <= 3, "bad activation code");
   NLT_CHECK_ARG(beta == 0.f || beta == 1.f, "beta must be 0 or 1");
-  if (k.M > 0 && pwd2s_applicable(k, bias, act, out, mask_y, &ex))
-    return launch_pwd2s_route(k, beta, mask_y, mask_act, out, (cudaStream_t)stream, &ex);
-  if (k.M == 0 || !pw_extra_applicable(k, ex, out, mask_y))
-    return set_err(NLT_ERR_UNSUPPORTED, "fused pointwise term: shape not served by the pointwise kernel");
-  return launch_pw_conv(k, bias, act, beta, mask_y, mask_act, out, (cudaStream_t)stream, &ex);
+  const Route r = fused_route(k, ex, bias, act, mask_y, out);
+  if (r == Route::NONE) return set_err(NLT_ERR_UNSUPPORTED, "fused pointwise term: shape not served by the pointwise kernel");
+  return launch_route(r, k, bias, act, beta, mask_y, mask_act, out, &ex, nullptr, 0, false, (cudaStream_t)stream);
 }
 
 int nlt_gconv_fwd(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
@@ -918,19 +1022,11 @@ int64_t nlt_gconv_wgrad_workspace_bytes(const nlt_gconv_desc* d) {
   GConvK ph[16];
   int np = 0;
   if (build_phases(d, ph, &np, /*allow_d2s=*/true) != NLT_OK) return -1;
-  if (np == 1 && ph[0].d2s && !pwx_wgrad_applicable(ph[0], nullptr) && !wop_wgrad_applicable(ph[0], nullptr) &&
-      !wgrad_small_applicable(ph[0]) &&
-      !use_tc_wgrad(ph[0]) && build_phases(d, ph, &np, false) != NLT_OK) return -1;
+  if (np == 1 && ph[0].d2s && !wgrad_keeps_d2s(ph[0], nullptr) && build_phases(d, ph, &np, false) != NLT_OK) return -1;
   size_t mx = 0;
   for (int i = 0; i < np; ++i) {
     if (ph[i].M == 0) continue;
-    size_t need = pwx_wgrad_applicable(ph[i], nullptr) ? pwx_wgrad_ws_floats(ph[i])
-                  : wop_wgrad_applicable(ph[i], nullptr) ? wop_wgrad_ws_floats(ph[i])
-                  : wopn_wgrad_applicable(ph[i], nullptr) ? wopn_wgrad_ws_floats(ph[i])
-                  : pws_wgrad_applicable(ph[i], nullptr) ? pws_wgrad_ws_floats(ph[i])
-                  : use_tc_wgrad(ph[i]) ? tc_wgrad_ws_floats(ph[i])
-                  : wgrad_tpp_applicable(ph[i]) ? wgrad_tpp_ws_floats(ph[i])
-                  : wgrad_small_applicable(ph[i]) ? wgrad_small_ws_floats(ph[i]) : plan_wgrad(ph[i]).ws_floats;
+    const size_t need = wgrad_ws_floats(wgrad_route(ph[i], nullptr, INT64_MAX), ph[i]);
     if (need > mx) mx = need;
   }
   return (int64_t)(mx * sizeof(float));
@@ -942,11 +1038,7 @@ int nlt_gconv_wgrad(const nlt_gconv_desc* d, const float* G, float* dW, float* d
   int np = 0;
   int rc = build_phases(d, ph, &np, /*allow_d2s=*/true);
   if (rc != NLT_OK) return rc;
-  // a k == stride transposed conv keeps its one-pass depth-to-space form when a kernel takes it (the warp-stream
-  // kernel for narrow tiles, the wgmma kernel from K_d = 128 up); otherwise s*s phases
-  if (np == 1 && ph[0].d2s && !pwx_wgrad_applicable(ph[0], G) && !wop_wgrad_applicable(ph[0], G) &&
-      !wgrad_small_applicable(ph[0]) && !use_tc_wgrad(ph[0]))
-    rc = build_phases(d, ph, &np, false);
+  if (np == 1 && ph[0].d2s && !wgrad_keeps_d2s(ph[0], G)) rc = build_phases(d, ph, &np, false);
   if (rc != NLT_OK) return rc;
   NLT_CHECK_ARG(G != nullptr && dW != nullptr && workspace != nullptr, "null pointer");
   cudaStream_t st = (cudaStream_t)stream;
@@ -957,48 +1049,35 @@ int nlt_gconv_wgrad(const nlt_gconv_desc* d, const float* G, float* dW, float* d
     float* ws = (float*)workspace;
     WgradK w;
     size_t KD_pad = 0;
-    if (pwx_wgrad_applicable(k, G) && (int64_t)(pwx_wgrad_ws_floats(k) * sizeof(float)) <= workspace_bytes) {
-      rc = launch_pwx_wgrad(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (wop_wgrad_applicable(k, G) && (int64_t)(wop_wgrad_ws_floats(k) * sizeof(float)) <= workspace_bytes) {
-      // few-channel layers at (near) full resolution: register-tile outer products, one warp per unit kind (nlt_wop.cu)
-      rc = launch_wop_wgrad(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (wopn_wgrad_applicable(k, G) && (int64_t)(wopn_wgrad_ws_floats(k) * sizeof(float)) <= workspace_bytes) {
-      // final 1x1 conv into <= 4 channels: coalesced (pixel, channel quad) lanes (nlt_wop.cu)
-      rc = launch_wopn_wgrad(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (pws_wgrad_applicable(k, G) && (int64_t)(pws_wgrad_ws_floats(k) * sizeof(float)) <= workspace_bytes) {
-      rc = launch_pws_wgrad(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (use_tc_wgrad(k)) {
-      NLT_CHECK_ARG((int64_t)(tc_wgrad_ws_floats(k) * sizeof(float)) <= workspace_bytes, "workspace too small");
-      rc = launch_tc_wgrad(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (wgrad_tpp_applicable(k)) {
-      NLT_CHECK_ARG((int64_t)(wgrad_tpp_ws_floats(k) * sizeof(float)) <= workspace_bytes, "workspace too small");
-      rc = launch_wgrad_tpp(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else if (wgrad_small_applicable(k)) {
-      NLT_CHECK_ARG((int64_t)(wgrad_small_ws_floats(k) * sizeof(float)) <= workspace_bytes, "workspace too small");
-      rc = launch_wgrad_small(k, G, ws, &w, &KD_pad, st);
-      if (rc != NLT_OK) return rc;
-    } else {
-      WgradPlan p = plan_wgrad(k);
-      NLT_CHECK_ARG((int64_t)(p.ws_floats * sizeof(float)) <= workspace_bytes, "workspace too small: need %lld have %lld",
-                    (long long)(p.ws_floats * sizeof(float)), (long long)workspace_bytes);
-      w.g = k; w.GS = p.GS; w.KG = p.KG; w.ld = p.ld; w.nsplit = p.nsplit; w.pix_per_split = p.pix_per_split;
-      KD_pad = p.KD_pad;
-      dim3 grid(p.kd_tiles, p.n_tiles, p.nsplit);
-      switch (p.tn) {
-        case 64: gconv_wgrad_kernel<32, 64, 8, 8, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
-        case 32: gconv_wgrad_kernel<32, 32, 8, 4, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
-        case 16: gconv_wgrad_kernel<32, 16, 4, 4, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
-        case 8: gconv_wgrad_kernel<32, 8, 4, 4, 64><<<grid, 64, 0, st>>>(w, G, ws); break;
-        default: gconv_wgrad_kernel<32, 4, 4, 4, 32><<<grid, 32, 0, st>>>(w, G, ws); break;
+    const WgradRoute r = wgrad_route(k, G, workspace_bytes);
+    const int64_t need = (int64_t)(wgrad_ws_floats(r, k) * sizeof(float));
+    NLT_CHECK_ARG(need <= workspace_bytes, "workspace too small: need %lld have %lld", (long long)need,
+                  (long long)workspace_bytes);
+    switch (r) {
+      case WgradRoute::PWX: rc = launch_pwx_wgrad(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::WOP: rc = launch_wop_wgrad(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::WOPN: rc = launch_wopn_wgrad(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::PWS: rc = launch_pws_wgrad(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::TC: rc = launch_tc_wgrad(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::TPP: rc = launch_wgrad_tpp(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::SMALL: rc = launch_wgrad_small(k, G, ws, &w, &KD_pad, st); break;
+      case WgradRoute::TILED: {
+        WgradPlan p = plan_wgrad(k);
+        w.g = k; w.GS = p.GS; w.KG = p.KG; w.ld = p.ld; w.nsplit = p.nsplit; w.pix_per_split = p.pix_per_split;
+        KD_pad = p.KD_pad;
+        dim3 grid(p.kd_tiles, p.n_tiles, p.nsplit);
+        switch (p.tn) {
+          case 64: gconv_wgrad_kernel<32, 64, 8, 8, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
+          case 32: gconv_wgrad_kernel<32, 32, 8, 4, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
+          case 16: gconv_wgrad_kernel<32, 16, 4, 4, 128><<<grid, 128, 0, st>>>(w, G, ws); break;
+          case 8: gconv_wgrad_kernel<32, 8, 4, 4, 64><<<grid, 64, 0, st>>>(w, G, ws); break;
+          default: gconv_wgrad_kernel<32, 4, 4, 4, 32><<<grid, 32, 0, st>>>(w, G, ws); break;
+        }
+        NLT_CUDA_LAUNCH_CHECK("gconv_wgrad_kernel");
+        break;
       }
-      NLT_CUDA_LAUNCH_CHECK("gconv_wgrad_kernel");
     }
+    if (rc != NLT_OK) return rc;
     // every phase sees a disjoint subset of lattice pixels, so the bias gradient
     // accumulates across phases; taps are disjoint across phases.
     const size_t total = (size_t)w.KG * 4 * k.Cout;

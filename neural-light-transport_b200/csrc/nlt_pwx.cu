@@ -391,15 +391,8 @@ static size_t pwx_wgrad_smem(const PwxParams& p) {
 constexpr size_t PWX_SMEM_MAX = 56 * 1024;      // four CTAs per SM
 constexpr size_t PWX_WGRAD_SMEM_MAX = 72 * 1024; // three CTAs per SM (K = 65 .. 96: the level-11 up-conv)
 
-int g_opt_pf_ns = -1, g_opt_pwx_ns = -1;     // options "pf_ns" / "pwx_ns": threads per pixel of the forward kernels
-int g_opt_pwx = -1;     // option "pwx" / NLT_PWX: 1 (default) the kernels of this file, 0 the general routes
-static bool pwx_enabled() {
-  if (g_opt_pwx < 0) { const char* e = getenv("NLT_PWX"); g_opt_pwx = (e && e[0] == '0') ? 0 : 1; }
-  return g_opt_pwx == 1;
-}
-
 bool pwx_fwd_applicable(const GConvK& k, float beta, const float* mask_y, const float* out) {
-  if (!pwx_enabled() || !pwx_shape_ok(k) || beta != 0.f || mask_y != nullptr || !aligned16(out)) return false;
+  if (!pwx_shape_ok(k) || beta != 0.f || mask_y != nullptr || !aligned16(out)) return false;
   PwxParams p;
   return pwx_build(k, false, &p, nullptr, nullptr, nullptr) && pwx_fwd_smem(p) <= PWX_SMEM_MAX;
 }
@@ -434,9 +427,7 @@ int launch_pwx_fwd(const GConvK& k, const float* bias, int act, float* out, cuda
   if (e == cudaSuccess)
     e = cudaMemcpyToSymbolAsync(pwx_cw, stage, (size_t)p.K4 * 2 * 16 * sizeof(float2), 0, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwx weight table: %s", cudaGetErrorString(e));
-  // NLT_PWX_NS: threads per pixel (default 1; 2 = the output split)
-  if (g_opt_pwx_ns < 0) { const char* e = getenv("NLT_PWX_NS"); g_opt_pwx_ns = (e && e[0] == '2') ? 2 : 1; }
-  const int ns = g_opt_pwx_ns;
+  const int ns = opt(Opt::PWX_NS);     // threads per pixel (default 1; 2 = the output split)
 #define PWX_GO(K4_) do { if (ns == 1) return pwx_fwd_launch<K4_, 1>(p, bias, act, out, smem, st); \
                          return pwx_fwd_launch<K4_, 2>(p, bias, act, out, smem, st); } while (0)
   switch (p.K4) {
@@ -556,7 +547,7 @@ static bool pwx_d2s_build(const GConvK& k, PwxParams* p) {
 }
 
 bool pwx_d2s_fwd_applicable(const GConvK& k, float beta, const float* mask_y, const float* out) {
-  if (!pwx_enabled() || !k.d2s || k.d2s_s != 2 || k.M == 0 || beta != 0.f || mask_y != nullptr || !aligned16(out)) return false;
+  if (!k.d2s || k.d2s_s != 2 || k.M == 0 || beta != 0.f || mask_y != nullptr || !aligned16(out)) return false;
   if ((k.cout_true != 4 && k.cout_true != 8) || k.Cout != 4 * k.cout_true) return false;
   if (k.ax.nt != k.Win || k.ay.nt != k.Hin || k.Hout != 2 * k.Hin || k.Wout != 2 * k.Win || k.Win % PWX_T != 0) return false;
   int K = 0;
@@ -765,21 +756,15 @@ pf_fwd_kernel(const PfParams p, const float* __restrict__ bias, const int act, f
   }
 }
 
-int g_opt_pf_s1 = -1;    // option "pf_s1" / NLT_PF_S1: the staged kernel also for the stride-1 16 -> 16 stencils (ahead of nlt_tiny.cu)
-int pf_s1_level() {
-  if (g_opt_pf_s1 < 0) { const char* e = getenv("NLT_PF_S1"); g_opt_pf_s1 = (e && e[0] == '1') ? 1 : 0; }
-  return g_opt_pf_s1;
-}
-
 static bool pf_build(const GConvK& k, PfParams* p, int* tp) {
   memset(p, 0, sizeof(*p));
-  if (!pwx_enabled() || k.d2s || k.M == 0) return false;
+  if (k.d2s || k.M == 0) return false;
   if (k.Cout != k.cout_true || (k.Cout != 16 && k.Cout != 32)) return false;
   if (k.ay.nu != 2 || k.ax.nu != 2 || k.ay.os != 1 || k.ax.os != 1 || k.ay.o0 != 0 || k.ax.o0 != 0) return false;
   const bool s1 = k.ay.it == 1 && k.ax.it == 1;
   if (s1) {
     // stride-1 2x2 stencil 16 -> 16 (second convs of level 1 / 10 and their adjoints), option "pf_s1"
-    if (pf_s1_level() <= 0 || k.nseg != 1 || k.seg[0].C != 16 || k.Cout != 16) return false;
+    if (k.nseg != 1 || k.seg[0].C != 16 || k.Cout != 16) return false;
     if (k.Hin != k.Hout || k.Win != k.Wout || k.ay.nt != k.Hout || k.ax.nt != k.Wout) return false;
     if ((k.ay.iu != 1 && k.ay.iu != -1) || (k.ax.iu != 1 && k.ax.iu != -1)) return false;
   } else {
@@ -852,9 +837,7 @@ int launch_pf_fwd(const GConvK& k, const float* bias, int act, float beta, const
   if (e == cudaSuccess)
     e = cudaMemcpyToSymbolAsync(pwx_cw, stage, (size_t)(p.K / 2) * k.Cout * sizeof(float2), 0, cudaMemcpyDeviceToDevice, st);
   if (e != cudaSuccess) return set_err(NLT_ERR_CUDA, "pwx weight table: %s", cudaGetErrorString(e));
-  // NLT_PF_NS: threads per pixel (default 1; 2 = the output split)
-  if (g_opt_pf_ns < 0) { const char* e = getenv("NLT_PF_NS"); g_opt_pf_ns = (e && e[0] == '2') ? 2 : 1; }
-  const int ns = g_opt_pf_ns;
+  const int ns = opt(Opt::PF_NS);      // threads per pixel (default 1; 2 = the output split)
 #define PF_GO(K4_, N_, TP_) \
   do { if (ns == 1) return pf_launch<K4_, N_, TP_, 1>(p, bias, act, out, beta, mask_y, mask_act, st); \
        return pf_launch<K4_, N_, TP_, 2>(p, bias, act, out, beta, mask_y, mask_act, st); } while (0)
@@ -878,7 +861,7 @@ static bool pwx_wgrad_d2s_ok(const GConvK& k) {
 }
 
 bool pwx_wgrad_applicable(const GConvK& k, const float* G) {
-  if (!pwx_enabled() || !(pwx_shape_ok(k) || pwx_wgrad_d2s_ok(k)) || (G != nullptr && !aligned16(G))) return false;
+  if (!(pwx_shape_ok(k) || pwx_wgrad_d2s_ok(k)) || (G != nullptr && !aligned16(G))) return false;
   PwxParams p;
   return pwx_build(k, true, &p, nullptr, nullptr, nullptr) && pwx_wgrad_smem(p) <= PWX_WGRAD_SMEM_MAX;
 }
@@ -1118,7 +1101,6 @@ static bool pwd_pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 bool pwd2s_applicable(const GConvK& k, const float* bias, int act, const float* out, const float* mask_y,
                       const PwExtra* ex) {
-  if (!pwx_enabled()) return false;
   if (!k.d2s || k.d2s_s != 2 || k.nseg != 1 || (k.cout_true != 16 && k.cout_true != 32) || k.Cout != 4 * k.cout_true ||
       k.M == 0) return false;
   const Seg& sg = k.seg[0];
@@ -1301,12 +1283,6 @@ pwd2s_mma_kernel(const PwdParams p) {
   }
 }
 
-int g_opt_pwmma = -1;   // option "pwmma" / NLT_PWMMA: 1 (default) the tensor-core kernels of this file, 0 the FMA ones
-bool pwmma_enabled() {
-  if (g_opt_pwmma < 0) { const char* e = getenv("NLT_PWMMA"); g_opt_pwmma = (e && e[0] == '0') ? 0 : 1; }
-  return g_opt_pwmma == 1;
-}
-
 template <int K, int CS>
 static int pwd2s_mma_launch(const PwdParams& p0, cudaStream_t st) {
   using C = PwmCfg<K, CS>;
@@ -1333,8 +1309,7 @@ int launch_pwd2s_mma(const GConvK& k, float beta, const float* mask_y, int mask_
                      const PwExtra* ex) {
   const int K = k.seg[0].C, CS = k.cout_true;
   PwdParams p = pwd_params(k, beta, mask_y, mask_act, out, ex);
-  if (g_opt_tc_rawhi < 0) { const char* e = getenv("NLT_TC_RAWHI"); g_opt_tc_rawhi = (e && e[0] == '0') ? 0 : 1; }
-  p.rawhi = g_opt_tc_rawhi;
+  p.rawhi = opt(Opt::TC_RAWHI);
   if (CS == 16) return K == 16 ? pwd2s_mma_launch<16, 16>(p, st) : pwd2s_mma_launch<32, 16>(p, st);
   return K == 32 ? pwd2s_mma_launch<32, 32>(p, st) : pwd2s_mma_launch<64, 32>(p, st);
 }
@@ -1510,7 +1485,7 @@ struct PwsPlan {
 static PwsPlan pws_plan(const GConvK& k) {
   PwsPlan pl;
   memset(&pl, 0, sizeof(pl));
-  if (!pwx_enabled() || k.d2s || k.M == 0) return pl;
+  if (k.d2s || k.M == 0) return pl;
   if (k.Cout != k.cout_true || (k.Cout != 16 && k.Cout != 32)) return pl;
   if (k.ay.nu != 2 || k.ax.nu != 2 || k.ay.iu != 1 || k.ax.iu != 1 || k.ay.i0 != 0 || k.ax.i0 != 0) return pl;
   if (k.ay.it != k.ax.it || (k.ay.it != 1 && k.ay.it != 2)) return pl;

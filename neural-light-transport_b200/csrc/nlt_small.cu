@@ -712,10 +712,6 @@ dconv_wide_kernel(const GConvK g, const float* __restrict__ bias, const int act,
   }
 }
 
-int g_opt_dconv_wide = -1;   // -1: environment default (NLT_DCONV_WIDE), 0 off, 1 on
-
-int g_opt_dconv_wide32 = -1;   // EXPERIMENTAL (not validated on hardware yet): the 32-output form, default off
-
 static bool dconv_wide_common(const GConvK& k, const float* out, const float* mask_y, int cout, int kmax, bool multi_seg) {
   if (k.d2s || k.M == 0) return false;
   if (k.Cout != cout || k.cout_true != k.Cout) return false;
@@ -732,27 +728,10 @@ static bool dconv_wide_common(const GConvK& k, const float* out, const float* ma
   return aligned16(out) && (mask_y == nullptr || aligned16(mask_y));
 }
 
-int g_opt_dconv_wide8 = -1;    // the 8-output form (up-conv levels 11-12); default on
-
 bool dconv_wide_applicable(const GConvK& k, const float* out, const float* mask_y) {
-  if (g_opt_dconv_wide < 0) {
-    const char* e = getenv("NLT_DCONV_WIDE");
-    g_opt_dconv_wide = e ? (atoi(e) != 0) : NLT_DCONV_WIDE_DEFAULT;
-  }
-  if (g_opt_dconv_wide32 < 0) {
-    const char* e = getenv("NLT_DCONV_WIDE32");
-    g_opt_dconv_wide32 = e ? atoi(e) : 0;
-  }
-  if (g_opt_dconv_wide8 < 0) {
-    const char* e = getenv("NLT_DCONV_WIDE8");
-    g_opt_dconv_wide8 = e ? atoi(e) : 1;
-  }
-  if (g_opt_dconv_wide && dconv_wide_common(k, out, mask_y, 16, PW_KMAX, false)) return true;
-  if (g_opt_dconv_wide32 > 0 && dconv_wide_common(k, out, mask_y, 32, DW_KMAX, true)) return true;
-  return g_opt_dconv_wide8 > 0 && dconv_wide_common(k, out, mask_y, 8, DW_KMAX, true);
+  return dconv_wide_common(k, out, mask_y, 16, PW_KMAX, false) || dconv_wide_common(k, out, mask_y, 32, DW_KMAX, true) ||
+         dconv_wide_common(k, out, mask_y, 8, DW_KMAX, true);
 }
-
-int g_opt_dconv_cw = -1;   // option "dconv_cw" / NLT_DCONV_CW: constant-memory weight table (default on)
 
 static int dconv_cw_fill(const GConvK& k, int qt, cudaStream_t st) {
   dconv_cw_pack_kernel<<<8, 256, 0, st>>>(k, qt);
@@ -769,8 +748,8 @@ static int dconv_cw_fill(const GConvK& k, int qt, cudaStream_t st) {
 
 int launch_dconv_wide(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act,
                       float* out, cudaStream_t st) {
-  if (g_opt_dconv_cw < 0) { const char* e = getenv("NLT_DCONV_CW"); g_opt_dconv_cw = (e && e[0] == '0') ? 0 : 1; }
-  if (g_opt_dconv_cw == 1 && (k.Cout == 16 || k.Cout == 8)) {
+  // option "dconv_cw": the weights of the 16- / 8-output forms from a constant-memory table
+  if (opt(Opt::DCONV_CW) == 1 && (k.Cout == 16 || k.Cout == 8)) {
     int rc = dconv_cw_fill(k, k.Cout / 4, st);
     if (rc != NLT_OK) return rc;
     if (k.Cout == 16) {
@@ -791,7 +770,7 @@ int launch_dconv_wide(const GConvK& k, const float* bias, int act, float beta, c
   } else if (k.Cout == 8) {                  // experimental: pixel x 8 outputs, four pixels per thread
     const unsigned grid = (k.M + PW_THREADS * 4 - 1) / (PW_THREADS * 4);
     dconv_wide_kernel<2, 4, 3><<<grid, PW_THREADS, 0, st>>>(k, bias, act, beta, mask_y, mask_act, out);
-  } else if (g_opt_dconv_wide32 == 2) {      // two pixels per thread: 8 FMAs per weight LDS.128, ~2 CTAs per SM
+  } else if (opt(Opt::DCONV_WIDE32) == 2) {      // two pixels per thread: 8 FMAs per weight LDS.128, ~2 CTAs per SM
     const unsigned grid = (k.M + PW_THREADS * 2 - 1) / (PW_THREADS * 2);
     dconv_wide_kernel<8, 2, 2><<<grid, PW_THREADS, 0, st>>>(k, bias, act, beta, mask_y, mask_act, out);
   } else {                                   // one pixel per thread: 4 FMAs per weight LDS.128, 3 CTAs per SM
@@ -1154,8 +1133,6 @@ wgrad_rows_kernel(const WgradK w, const float* __restrict__ G, float* __restrict
   for (int i = tid; i < ROWS * LD; i += WS_THREADS) dst[i] = tile[i];
 }
 
-int g_opt_wgrad_rows = 1;
-
 static bool wgrad_rows_ok(const GConvK& k, const float* G) {
   if (k.cout_true % 4 != 0 || k.Cout % 4 != 0 || !aligned16(G)) return false;
   for (int s = 0; s < k.nseg; ++s)
@@ -1398,7 +1375,7 @@ int launch_wgrad_small(const GConvK& k, const float* G, float* ws, WgradK* w, si
   w->g = k; w->GS = pl.GS; w->KG = pl.KG; w->ld = pl.ld; w->nsplit = pl.nsplit; w->pix_per_split = pl.pps;
   *KD_pad = pl.KD_pad;
   const unsigned grid = pl.nsplit;
-  const bool rows = g_opt_wgrad_rows == 1 && wgrad_rows_ok(k, G);
+  const bool rows = opt(Opt::WGRAD_ROWS) == 1 && wgrad_rows_ok(k, G);   // option "wgrad_rows"; 0: flat-pixel form
   const uint32_t cpr = ((uint32_t)k.ax.nt + WR_CHUNK - 1) / WR_CHUNK;
   const uint32_t nchunks = (uint32_t)k.N * (uint32_t)k.ay.nt * cpr;
   // P <= 2 wants occupancy (128 registers, 4 CTAs per SM), the wide

@@ -32,8 +32,6 @@ constexpr int TC_THREADS = 384;                 // producer warpgroup + two cons
 constexpr uint32_t TC_SPIN_LIMIT = 1u << 28;    // watchdog: trap instead of hanging the GPU
 unsigned long long g_tc_launches = 0;           // tensor-core kernel launches (diagnostic)
 
-int g_opt_tc_rawhi = -1;
-
 struct TcParams {
   // lattice / tiling
   int N, Hl, Wl;            // lattice size (pixels this kernel enumerates)
@@ -526,22 +524,15 @@ static int pick_bn(int cout) {
   return 0;
 }
 
-// option "tc" = 2 (A/B testing): every shape the kernel can run takes it, ignoring the size heuristics below
-int g_tc_force = 0;
-
-// "tcs" (option / NLT_TCS): 1 = RS form (A operand split in registers), 0 = SS form (hi / lo planes in shared memory)
-int g_opt_tcs = -1;
-static bool tcs_enabled() {
-  if (g_opt_tcs < 0) { const char* e = getenv("NLT_TCS"); g_opt_tcs = e ? (atoi(e) != 0) : NLT_TCS_DEFAULT; }
-  return g_opt_tcs == 1;
-}
-
 // Which single-phase GConvK shapes the tensor path takes (everything else stays on the SIMT kernels).
 static TcPlan tc_plan(const GConvK& k) {
   TcPlan pl;
   memset(&pl, 0, sizeof(pl));
   pl.ok = false;
-  const bool ts = tcs_enabled();
+  // option "tcs": 1 = RS form (A operand split in registers), 0 = SS form (hi / lo planes in shared memory)
+  const bool ts = opt(Opt::TCS) == 1;
+  // option "tc" = 2 (A/B testing): every shape the kernel can run takes it, ignoring the size heuristics below
+  const bool force = opt(Opt::TC) == 2;
   pl.ts = ts;
   if (k.cout_true % 4 != 0) return pl;
   pl.bn = pick_bn(k.Cout);
@@ -556,7 +547,7 @@ static TcPlan tc_plan(const GConvK& k) {
   }
   const int TC_KB = pl.kbw;
   if (!aligned16(k.w)) { /* weights are only read by the pack kernel: no alignment needed */ }
-  if (!g_tc_force) {
+  if (!force) {
     // with less than 64 contraction terms the op is a pure stream: the pointwise / fp32 kernels are faster there
     if (k.ay.nu * k.ax.nu * ctot < 64) return pl;
     // 16-channel (64-byte-row) K-blocks only from K = 128 up: below that the FFMA stream kernels take these layers
@@ -574,7 +565,7 @@ static TcPlan tc_plan(const GConvK& k) {
   p.TW = TC_BM;
   while (p.TW / 2 >= p.Wl) p.TW /= 2;
   p.TH = TC_BM / p.TW;
-  if (!g_tc_force && (p.Wl % p.TW != 0 || p.Hl % p.TH != 0)) return pl;
+  if (!force && (p.Wl % p.TW != 0 || p.Hl % p.TH != 0)) return pl;
   p.tiles_x = (p.Wl + p.TW - 1) / p.TW; p.tiles_y = (p.Hl + p.TH - 1) / p.TH;
   // coordinate map
   const bool stride1 = (k.ay.it == 1 && k.ax.it == 1);
@@ -596,9 +587,8 @@ static TcPlan tc_plan(const GConvK& k) {
   p.d2s = k.d2s; p.d2s_s = k.d2s_s;
   // few output tiles: narrower column tiles so that more SMs get work (A is re-read from L2), but only while the finer
   // tiling still fits ONE wave of persistent CTAs: every tile pays the pipeline fill / drain of the kernel again
-  // (NLT_TC_SPLIT_WAVES=1: split whenever there are fewer tiles than SMs)
-  static int split_waves = -1;
-  if (split_waves < 0) { const char* e = getenv("NLT_TC_SPLIT_WAVES"); split_waves = (e && e[0] == '1') ? 1 : 0; }
+  // (option "tc_split_waves" = 1: split whenever there are fewer tiles than SMs)
+  const bool split_waves = opt(Opt::TC_SPLIT_WAVES) == 1;
   while (pl.bn > 32) {
     const long long tiles = (long long)p.N * p.tiles_x * p.tiles_y * (k.Cout / pl.bn);
     if (split_waves ? tiles >= sm_count() : 2 * tiles > sm_count()) break;
@@ -622,8 +612,7 @@ static TcPlan tc_plan(const GConvK& k) {
     pl.smem_bytes = (size_t)st * stage_bytes + TC_EPI_BYTES + 1024;
   }
   if (get_encode() == nullptr) return pl;
-  if (g_opt_tc_rawhi < 0) { const char* e = getenv("NLT_TC_RAWHI"); g_opt_tc_rawhi = (e && e[0] == '0') ? 0 : 1; }
-  p.rawhi = g_opt_tc_rawhi;
+  p.rawhi = opt(Opt::TC_RAWHI);
   pl.ok = true;
   return pl;
 }

@@ -114,14 +114,8 @@ tiny_stencil_kernel(const TinyParams p) {
   }
 }
 
-int g_opt_tiny = -1;     // option "tiny" / NLT_TINY: 1 (default) these kernels, 0 the general small-stencil routes
-static bool tiny_enabled() {
-  if (g_opt_tiny < 0) { const char* e = getenv("NLT_TINY"); g_opt_tiny = (e && e[0] == '0') ? 0 : 1; }
-  return g_opt_tiny == 1;
-}
-
 bool tiny_stencil_applicable(const GConvK& k, const float* out, const float* mask_y) {
-  if (!tiny_enabled() || k.d2s || k.M == 0 || k.nseg != 1) return false;
+  if (k.d2s || k.M == 0 || k.nseg != 1) return false;
   const Seg& sg = k.seg[0];
   if (!sg.vec || sg.sub != nullptr || sg.bcast) return false;
   if (sg.C != k.Cout || k.Cout != k.cout_true || (k.Cout != 4 && k.Cout != 8 && k.Cout != 16)) return false;

@@ -139,15 +139,6 @@ wop_wgrad_kernel(const __grid_constant__ WopParams p, float* __restrict__ ws) {
     }
 }
 
-// option "wop" / NLT_WOP: 0 off; 1 (default) the 4 -> 4 and 8 -> 8 stencils; 2 also the 16 -> 16 stencils and the
-// up-convs, which are correct but slower than the staged-patch / wgmma kernels (16 warps/SM at 128 registers cannot
-// hide the load latency)
-int g_opt_wop = -1;
-static int wop_level() {
-  if (g_opt_wop < 0) { const char* e = getenv("NLT_WOP"); g_opt_wop = e ? atoi(e) : 1; }
-  return g_opt_wop;
-}
-
 struct WopPlan {
   bool ok;
   WopParams p;
@@ -161,8 +152,7 @@ static bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 static WopPlan wop_plan(const GConvK& k, const float* G) {
   WopPlan pl;
   memset(&pl, 0, sizeof(pl));
-  if (wop_level() <= 0 || k.M == 0) return pl;
-  if (wop_level() < 2 && (k.d2s || k.Cout > 8)) return pl;
+  if (k.M == 0) return pl;
   WopParams& p = pl.p;
   for (int s = 0; s < k.nseg; ++s)
     if (!k.seg[s].vec || k.seg[s].sub != nullptr || k.seg[s].bcast) return pl;
@@ -412,7 +402,6 @@ static bool wopn_plan(const GConvK& k, const float* G, WopnParams* p, unsigned* 
 }
 
 bool wopn_wgrad_applicable(const GConvK& k, const float* G) {
-  if (wop_level() <= 0) return false;
   WopnParams p; unsigned grid; int GS;
   return wopn_plan(k, G, &p, &grid, &GS);
 }

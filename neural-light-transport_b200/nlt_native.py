@@ -3,6 +3,7 @@
 The product path has NO CPU fallback: if the shared library is missing or a
 tensor is not a CUDA fp32 contiguous tensor, this module raises.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -49,6 +50,7 @@ _SIGS = {
     'nlt_version': (C.c_char_p, []),
     'nlt_last_error': (C.c_char_p, []),
     'nlt_set_option': (C.c_int, [C.c_char_p, C.c_int]),
+    'nlt_get_option': (C.c_int, [C.c_char_p, C.POINTER(C.c_int)]),
     'nlt_launch_count': (C.c_uint64, []),
     'nlt_tc_launch_count': (C.c_uint64, []),
     'nlt_kernel_launch_count': (C.c_uint64, [C.c_char_p]),
@@ -163,5 +165,26 @@ def tc_launch_count():
 
 
 def set_option(name, value):
-    """'tc' / 'tc_wgrad': 1 = wgmma 3xTF32 kernels where eligible (default), 0 = fp32-FMA kernels only."""
+    """Sets a process-wide kernel switch (the option table of csrc/nlt_gconv.cu), e.g. 'tc': 1 = wgmma 3xTF32 kernels
+    where eligible (default), 0 = fp32-FMA kernels only."""
     check(lib().nlt_set_option(name.encode(), int(value)))
+
+
+def get_option(name):
+    """Current value of a kernel switch: what set_option stored, else its environment value or default."""
+    v = C.c_int()
+    check(lib().nlt_get_option(name.encode(), C.byref(v)))
+    return v.value
+
+
+@contextlib.contextmanager
+def options(**kv):
+    """Sets the named switches for the duration of the block and restores their previous values on exit."""
+    saved = {k: get_option(k) for k in kv}
+    try:
+        for k, v in kv.items():
+            set_option(k, v)
+        yield
+    finally:
+        for k, v in saved.items():
+            set_option(k, v)

@@ -475,11 +475,6 @@ def poison_workspaces():
         todo += list(ws.subs.values())
 
 
-def _default_options():
-    import nlt_native as nat
-    nat.set_option('tc', 0 if os.environ.get('NLT_DISABLE_TC') == '1' else 1)
-
-
 def check_routes(arm, got):
     path = os.path.join(ROUTES_DIR, '%s.json' % arm)
     if os.environ.get('NLT_UPDATE_ROUTES') == '1':
@@ -552,9 +547,7 @@ def test_census_of_the_benchmarked_step(arm, monkeypatch):
     wl = bench.WORKLOADS[wl_name]
     uv = wl['uv']
     t0 = time.perf_counter()
-    for k, v in opts.items():
-        nat.set_option(k, v)
-    try:
+    with nat.options(**opts):
         model = models.get_model_class('nlt')(bench.make_config(wl))
         model.register_trainable()
         model.build(5 + wl['c_extra'], 3)
@@ -581,8 +574,6 @@ def test_census_of_the_benchmarked_step(arm, monkeypatch):
         torch.cuda.synchronize()
         census.finish_wgrad()
         torch.cuda.synchronize()
-    finally:
-        _default_options()
     seconds = time.perf_counter() - t0
     routes = census.route_table()
     rec = {'arm': arm, 'workload': wl_name, 'batch': B, 'options': opts, 'tau': TAU, 'census_seconds': seconds,

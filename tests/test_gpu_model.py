@@ -72,9 +72,8 @@ def path(request):
     """Runs a test on both execution paths of the library: 'fp32' = fp32-FMA kernels only (strict parity
     bar), 'tc' = wgmma 3xTF32 kernels wherever a shape is eligible (the default, performance path)."""
     import nlt_native as nat
-    nat.set_option('tc', 1 if request.param == 'tc' else 0)
-    yield request.param
-    nat.set_option('tc', 1)
+    with nat.options(tc=1 if request.param == 'tc' else 0):
+        yield request.param
 
 
 CASES = [
@@ -222,27 +221,26 @@ def test_train_steps_match_oracle_amsgrad():
     m/sqrt(v) turns a derivative-bit flip into an O(lr) parameter difference)."""
     import trainvali
     import nlt_native as nat
-    nat.set_option('tc', 0)
-    from util import synth
-    m, cfg = make_model(uvh=64, uvw=64, imh=64, imw=64, depth=64)
-    oc = ocfg(cfg)
-    params = O.init_params(oc, seed=13, dtype=torch.float64)
-    m.build(5, 3)
-    m.load_params(params)
-    strategy = trainvali.Strategy()
-    opt = trainvali.Adam(learning_rate=1e-3, amsgrad=True)
-    st = {k: [torch.zeros_like(v) for _ in range(3)] for k, v in params.items()}
-    for step in range(1, 4):
-        bt = synth.make_batch(2, 64, 64, seed=100 + step)
-        loss, _ = trainvali.distributed_train_step(strategy, m, bt, opt, 2)
-        ps = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
-        l64 = O.train_loss(ps, oc, tuple(t.double() if torch.is_tensor(t) else t for t in bt), 2)
-        l64.backward()
-        assert abs(float(loss) - float(l64)) <= 1e-4 * abs(float(l64))
-        for k in params:
-            p, mm, v, vh = O.amsgrad_step(params[k], ps[k].grad, *st[k], step, 1e-3)
-            params[k], st[k] = p, [mm, v, vh]
-    nat.set_option('tc', 1)
+    with nat.options(tc=0):
+        from util import synth
+        m, cfg = make_model(uvh=64, uvw=64, imh=64, imw=64, depth=64)
+        oc = ocfg(cfg)
+        params = O.init_params(oc, seed=13, dtype=torch.float64)
+        m.build(5, 3)
+        m.load_params(params)
+        strategy = trainvali.Strategy()
+        opt = trainvali.Adam(learning_rate=1e-3, amsgrad=True)
+        st = {k: [torch.zeros_like(v) for _ in range(3)] for k, v in params.items()}
+        for step in range(1, 4):
+            bt = synth.make_batch(2, 64, 64, seed=100 + step)
+            loss, _ = trainvali.distributed_train_step(strategy, m, bt, opt, 2)
+            ps = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
+            l64 = O.train_loss(ps, oc, tuple(t.double() if torch.is_tensor(t) else t for t in bt), 2)
+            l64.backward()
+            assert abs(float(loss) - float(l64)) <= 1e-4 * abs(float(l64))
+            for k in params:
+                p, mm, v, vh = O.amsgrad_step(params[k], ps[k].grad, *st[k], step, 1e-3)
+                params[k], st[k] = p, [mm, v, vh]
     got = m.export_params()
     for k in params:
         assert float((got[k].double().cpu() - params[k]).abs().max()) <= 5e-5, k

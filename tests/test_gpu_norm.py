@@ -50,8 +50,7 @@ def test_model_with_norm_forward_backward(kind):
     applies unchanged, so the strict bars are used on the activation-branch-agnostic quantities)."""
     import nlt_native as nat
     from util import synth
-    nat.set_option('tc', 0)
-    try:
+    with nat.options(tc=0):
         m, cfg = make_model(uvh=64, uvw=64, imh=64, imw=64, norm=kind)
         oc = ocfg(cfg)
         B = 2
@@ -68,8 +67,6 @@ def test_model_with_norm_forward_backward(kind):
         m.set_loss_grad_scale(1.0 / B)
         m.compute_loss(pred, gt, **kw)
         m.backward()
-    finally:
-        nat.set_option('tc', 1)
     assert float((pred.double().cpu() - p64.detach()).abs().max()) <= 5e-5
     grads = m.export_grads()
     assert set(grads) == set(params)

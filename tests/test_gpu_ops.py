@@ -3,8 +3,6 @@ oracle on seeded inputs.  Tolerances are fp32 round-off of sums of K terms
 (the SIMT path is plain fp32 FMA; no tensor-core truncation)."""
 import ctypes as C
 
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -177,11 +175,8 @@ def test_outer_product_wgrad_all_shapes(kind, k, s, H, W, segc, cout):
     """nlt_wop.cu also serves the up-convs and the 16 -> 16 stencils (option wop = 2; off by default because the
     staged-patch / wgmma kernels are faster there): same oracle check as every other route."""
     import nlt_native as nat
-    nat.set_option('wop', 2)
-    try:
+    with nat.options(wop=2):
         test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
-    finally:
-        nat.set_option('wop', int(os.environ.get('NLT_WOP', '1')))
 
 
 NS2_SHAPES = [g for g in GEOMS if g[6] in (16, 32) and g[4] >= 128 and (
@@ -193,15 +188,8 @@ def test_two_threads_per_pixel_forward_kernels(kind, k, s, H, W, segc, cout):
     """The pointwise / staged-patch forward kernels also exist with two threads per pixel (options pwx_ns / pf_ns = 2,
     off by default): same oracle check."""
     import nlt_native as nat
-    nat.set_option('pwx_ns', 2)
-    nat.set_option('pf_ns', 2)
-    nat.set_option('pf', 1)
-    try:
+    with nat.options(pwx_ns=2, pf_ns=2, pf=1):
         test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
-    finally:
-        nat.set_option('pwx_ns', 1)
-        nat.set_option('pf_ns', 1)
-        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
 
 
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', [('conv', 2, 2, 4, 512, [16], 32), ('conv', 2, 2, 4, 256, [32], 16),
@@ -214,15 +202,10 @@ def test_staged_patch_forward_and_pwd2s_first_routes(kind, k, s, H, W, segc, cou
     into 16- / 32-channel sources: pwd2s_kernel)."""
     import nlt_native as nat
     kernel = 'pf_fwd_kernel' if H in (4, 6) else 'pwd2s_kernel'
-    nat.set_option('pf', 1)
-    nat.set_option('pwd2s_first', 1)
-    try:
+    with nat.options(pf=1, pwd2s_first=1):
         n0 = nat.kernel_launch_count(kernel)
         test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
         assert nat.kernel_launch_count(kernel) > n0, kernel + ' did not run'
-    finally:
-        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
-        nat.set_option('pwd2s_first', int(os.environ.get('NLT_PWD2S_FIRST', '0')))
 
 
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', [('conv', 2, 1, 5, 128, [16], 16), ('deconv', 2, 1, 5, 256, [16], 16),
@@ -231,16 +214,11 @@ def test_staged_patch_kernel_on_stride1_stencils(kind, k, s, H, W, segc, cout):
     """pf_fwd_kernel in its stride-1 form (option pf_s1): forward and input gradient of the 16 -> 16 2x2 stencils,
     SAME padding on either side (conv / deconv flavour)."""
     import nlt_native as nat
-    nat.set_option('pf_s1', 1)
-    nat.set_option('pf', 1)
-    try:
+    with nat.options(pf_s1=1, pf=1):
         for act in ('leakyrelu', None):
             n0 = nat.kernel_launch_count('pf_fwd_kernel')
             test_gconv_forward_backward(kind, k, s, H, W, segc, cout, act)
             assert nat.kernel_launch_count('pf_fwd_kernel') > n0, 'pf_fwd_kernel did not run'
-    finally:
-        nat.set_option('pf_s1', int(os.environ.get('NLT_PF_S1', '0')))
-        nat.set_option('pf', int(os.environ.get('NLT_PF', '0')))
 
 
 TC_SHAPES = [g for g in GEOMS if all(c % 16 == 0 for c in g[5]) and g[6] % 16 == 0 and g[3] * g[4] >= 256]
@@ -253,16 +231,11 @@ def test_tensor_core_raw_hi_operand(kind, k, s, H, W, segc, cout):
     rounding) or, with 0, rounded to TF32.  Same oracle check, same tolerance for both splits; option tc = 2 puts every
     shape on the wgmma kernel, and its launch counter must move."""
     import nlt_native as nat
-    nat.set_option('tc', 2)
-    try:
-        for v in (1, 0):         # default form, and the one that rounds hi
-            nat.set_option('tc_rawhi', v)
+    for v in (1, 0):         # default form, and the one that rounds hi
+        with nat.options(tc=2, tc_rawhi=v):
             n0 = nat.tc_launch_count()
             test_gconv_forward_backward(kind, k, s, H, W, segc, cout, 'leakyrelu')
             assert nat.tc_launch_count() > n0, 'tensor-core kernel did not run'
-    finally:
-        nat.set_option('tc_rawhi', int(os.environ.get('NLT_TC_RAWHI', '1')))
-        nat.set_option('tc', 1)
 
 
 @pytest.fixture(params=['ss', 'ts'])
@@ -270,12 +243,8 @@ def tc_form(request):
     """Both forms of the wgmma forward / input-gradient kernel: 'ss' = hi / lo activation planes written to shared
     memory (both operands from shared memory), 'ts' = the activation operand split in registers (wgmma RS form)."""
     import nlt_native as nat
-    nat.set_option('tcs', 1 if request.param == 'ts' else 0)
-    yield request.param
-    nat.set_option('tcs', int(os.environ.get('NLT_TCS', '%d' % TCS_DEFAULT)))
-
-
-TCS_DEFAULT = 1
+    with nat.options(tcs=1 if request.param == 'ts' else 0):
+        yield request.param
 
 
 @pytest.mark.parametrize('kind,k,s,H,W,segc,cout', TC_SHAPES)
@@ -292,21 +261,20 @@ def test_tensor_core_vs_fp32_kernels(kind, k, s, H, W, segc, cout, tc_form):
     dzs = None
     res = {}
     for mode in ('tc', 'fp32'):
-        nat.set_option('tc', 2 if mode == 'tc' else 0)
-        L = engine.ConvLayer(kind, k, s, cout, 'leakyrelu')
-        L.build(sum(segc), dev, torch.Generator().manual_seed(1))
-        L.bias.copy_(torch.linspace(-0.1, 0.1, cout, device=dev))
-        acts = [engine.Act(x, act='leakyrelu', needs_grad=True) for x in xs]
-        tape = engine.Tape()
-        t0 = nat.tc_launch_count()
-        y = L.forward([engine.Seg(a) for a in acts], tape)
-        if dzs is None:
-            dzs = torch.randn_like(y.t)
-        y.grad = dzs.clone()
-        tape.backward()
-        res[mode] = dict(y=y.t.clone(), gk=L.gkernel.clone(), gb=L.gbias.clone(), gx=[a.grad.clone() for a in acts],
-                         tc=nat.tc_launch_count() - t0)
-    nat.set_option('tc', 1)
+        with nat.options(tc=2 if mode == 'tc' else 0):
+            L = engine.ConvLayer(kind, k, s, cout, 'leakyrelu')
+            L.build(sum(segc), dev, torch.Generator().manual_seed(1))
+            L.bias.copy_(torch.linspace(-0.1, 0.1, cout, device=dev))
+            acts = [engine.Act(x, act='leakyrelu', needs_grad=True) for x in xs]
+            tape = engine.Tape()
+            t0 = nat.tc_launch_count()
+            y = L.forward([engine.Seg(a) for a in acts], tape)
+            if dzs is None:
+                dzs = torch.randn_like(y.t)
+            y.grad = dzs.clone()
+            tape.backward()
+            res[mode] = dict(y=y.t.clone(), gk=L.gkernel.clone(), gb=L.gbias.clone(),
+                             gx=[a.grad.clone() for a in acts], tc=nat.tc_launch_count() - t0)
     assert res['fp32']['tc'] == 0
     assert res['tc']['tc'] > 0
     rel = lambda a, b: float((a.double() - b.double()).norm() / b.double().norm())
@@ -332,10 +300,8 @@ def test_wgrad_row_run_vs_flat_pixel_kernel(kind, k, s, H, W, segc, cout):
     xs = [torch.randn(N, H, W, c, device=dev) for c in segc]
     dzs = None
     res = {}
-    nat.set_option('tc', 0)
-    try:
-        for mode in (1, 0):
-            nat.set_option('wgrad_rows', mode)
+    for mode in (1, 0):
+        with nat.options(tc=0, wgrad_rows=mode):
             L = engine.ConvLayer(kind, k, s, cout, 'leakyrelu')
             L.build(sum(segc), dev, torch.Generator().manual_seed(1))
             acts = [engine.Act(x, act='leakyrelu', needs_grad=True) for x in xs]
@@ -346,9 +312,6 @@ def test_wgrad_row_run_vs_flat_pixel_kernel(kind, k, s, H, W, segc, cout):
             y.grad = dzs.clone()
             tape.backward()
             res[mode] = (L.gkernel.clone(), L.gbias.clone())
-    finally:
-        nat.set_option('wgrad_rows', 1)
-        nat.set_option('tc', 1)
     rel = lambda a, b: float((a.double() - b.double()).norm() / b.double().norm())
     assert rel(res[1][0], res[0][0]) <= 1e-5
     assert rel(res[1][1], res[0][1]) <= 1e-5
@@ -427,10 +390,8 @@ def test_wide_stencil_32_outputs(kind, k, s, H, W, cin, mode):
     torch.manual_seed(31)
     x = torch.randn(3, H, W, cin, device=dev)
     res = {}
-    nat.set_option('tc', 0)
-    try:
-        for m in (mode, 0):
-            nat.set_option('dconv_wide32', m)
+    for m in (mode, 0):
+        with nat.options(tc=0, dconv_wide32=m):
             L = engine.ConvLayer(kind, k, s, 32, 'leakyrelu')
             L.build(cin, dev, torch.Generator().manual_seed(1))
             L.bias.copy_(torch.linspace(-0.1, 0.1, 32, device=dev))
@@ -441,9 +402,6 @@ def test_wide_stencil_32_outputs(kind, k, s, H, W, cin, mode):
             y.grad = torch.randn_like(y.t)
             tape.backward()
             res[m] = (y.t.clone(), a.grad.clone(), L.gkernel.clone())
-    finally:
-        nat.set_option('dconv_wide32', 0)
-        nat.set_option('tc', 1)
     rel = lambda p, q: float((p.double() - q.double()).norm() / q.double().norm())
     assert rel(res[mode][0], res[0][0]) <= 1e-5
     assert rel(res[mode][1], res[0][1]) <= 1e-5
@@ -460,10 +418,8 @@ def test_wide_stencil_preferred_over_quad_kernel(kind, k, s, H, W, cin):
     torch.manual_seed(33)
     x = torch.randn(3, H, W, cin, device=dev)
     res = {}
-    nat.set_option('tc', 0)
-    try:
-        for m in (1, 0):
-            nat.set_option('dconv_wide_first', m)
+    for m in (1, 0):
+        with nat.options(tc=0, dconv_wide_first=m):
             L = engine.ConvLayer(kind, k, s, 16, 'leakyrelu')
             L.build(cin, dev, torch.Generator().manual_seed(1))
             a = engine.Act(x, act='leakyrelu', needs_grad=True)
@@ -473,9 +429,6 @@ def test_wide_stencil_preferred_over_quad_kernel(kind, k, s, H, W, cin):
             y.grad = torch.randn_like(y.t)
             tape.backward()
             res[m] = (y.t.clone(), a.grad.clone())
-    finally:
-        nat.set_option('dconv_wide_first', 1)      # library default
-        nat.set_option('tc', 1)
     rel = lambda p, q: float((p.double() - q.double()).norm() / q.double().norm())
     assert rel(res[1][0], res[0][0]) <= 1e-5 and rel(res[1][1], res[0][1]) <= 1e-5
 
@@ -491,11 +444,8 @@ def test_wide_stencil_8_outputs_and_virtual_concats(kind, k, s, H, W, segc, cout
     torch.manual_seed(35)
     xs = [torch.randn(3, H, W, c, device=dev) for c in segc]
     res = {}
-    nat.set_option('tc', 0)
-    try:
-        for m in (1, 0):
-            for opt in ('dconv_wide8', 'dconv_wide32', 'dconv_wide_first'):
-                nat.set_option(opt, m)
+    for m in (1, 0):
+        with nat.options(tc=0, dconv_wide8=m, dconv_wide32=m, dconv_wide_first=m):
             L = engine.ConvLayer(kind, k, s, cout, 'leakyrelu')
             L.build(sum(segc), dev, torch.Generator().manual_seed(1))
             acts = [engine.Act(x, act='leakyrelu', needs_grad=True) for x in xs]
@@ -505,10 +455,6 @@ def test_wide_stencil_8_outputs_and_virtual_concats(kind, k, s, H, W, segc, cout
             y.grad = torch.randn_like(y.t)
             tape.backward()
             res[m] = [y.t.clone()] + [a.grad.clone() for a in acts]
-    finally:
-        for opt, dflt in (('dconv_wide8', 1), ('dconv_wide32', 0), ('dconv_wide_first', 1)):
-            nat.set_option(opt, dflt)                 # library defaults
-        nat.set_option('tc', 1)
     rel = lambda p, q: float((p.double() - q.double()).norm() / q.double().norm())
     for p, q in zip(res[1], res[0]):
         assert rel(p, q) <= 1e-5

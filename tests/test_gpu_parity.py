@@ -110,21 +110,21 @@ def test_default_path_meets_the_strict_gradient_bar_given_its_own_relu_branches(
     the strict bar in test_gpu_model.py is therefore the handful of derivative bits that flip where a pre-activation
     lies within ~1e-6 of zero; their number is recorded and bounded."""
     import nlt_native as nat
-    nat.set_option('tc', 1)
-    B = 2
-    m, oc, bt, params, masks, pred, per = _product_and_masks(over, B, seed=1234, c_extra=c_extra)
-    p64, g_masked, flips = _oracle_grads(params, oc, bt, B, masks)
-    _, g_plain, _ = _oracle_grads(params, oc, bt, B)
-    assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
-    grads = m.export_grads()
-    worst_masked = max(rel_fro(grads[k], g_masked[k]) for k in params)
-    worst_plain = max(rel_fro(grads[k], g_plain[k]) for k in params)
-    frac = flips['flipped'] / max(flips['total'], 1)
-    _record('tc_masks_cq%d' % (5 + c_extra), {'worst_rel_fro_with_product_masks': worst_masked,
-                                             'worst_rel_fro_plain_oracle': worst_plain, 'flipped_bits': flips['flipped'],
-                                             'activation_elements': flips['total'], 'flipped_fraction': frac})
-    assert worst_masked <= 1e-4, (worst_masked, worst_plain, flips)
-    assert frac <= 1e-4, flips        # a few bits in a million elements, all at |pre-activation| ~ 1e-6
+    with nat.options(tc=1):
+        B = 2
+        m, oc, bt, params, masks, pred, per = _product_and_masks(over, B, seed=1234, c_extra=c_extra)
+        p64, g_masked, flips = _oracle_grads(params, oc, bt, B, masks)
+        _, g_plain, _ = _oracle_grads(params, oc, bt, B)
+        assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
+        grads = m.export_grads()
+        worst_masked = max(rel_fro(grads[k], g_masked[k]) for k in params)
+        worst_plain = max(rel_fro(grads[k], g_plain[k]) for k in params)
+        frac = flips['flipped'] / max(flips['total'], 1)
+        _record('tc_masks_cq%d' % (5 + c_extra), {'worst_rel_fro_with_product_masks': worst_masked,
+                                                 'worst_rel_fro_plain_oracle': worst_plain, 'flipped_bits': flips['flipped'],
+                                                 'activation_elements': flips['total'], 'flipped_fraction': frac})
+        assert worst_masked <= 1e-4, (worst_masked, worst_plain, flips)
+        assert frac <= 1e-4, flips        # a few bits in a million elements, all at |pre-activation| ~ 1e-6
 
 
 def test_three_amsgrad_steps_on_the_default_path():
@@ -135,42 +135,42 @@ def test_three_amsgrad_steps_on_the_default_path():
     import trainvali
     import nlt_native as nat
     from util import synth
-    nat.set_option('tc', 1)
-    m, cfg = make_model(uvh=64, uvw=64, imh=64, imw=64, depth=64)
-    oc = ocfg(cfg)
-    params = O.init_params(oc, seed=13, dtype=torch.float64)
-    init = {k: v.clone() for k, v in params.items()}
-    m.build(5, 3)
-    m.load_params(params)
-    strategy = trainvali.Strategy()
-    opt = trainvali.Adam(learning_rate=1e-3, amsgrad=True)
-    st = {k: [torch.zeros_like(v) for _ in range(3)] for k, v in params.items()}
-    loss_rel = []
-    for step in range(1, 4):
-        bt = synth.make_batch(2, 64, 64, seed=100 + step)
-        loss, _ = trainvali.distributed_train_step(strategy, m, bt, opt, 2)
-        ps = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
-        l64 = O.train_loss(ps, oc, tuple(t.double() if torch.is_tensor(t) else t for t in bt), 2)
-        l64.backward()
-        loss_rel.append(abs(float(loss) - float(l64)) / abs(float(l64)))
+    with nat.options(tc=1):
+        m, cfg = make_model(uvh=64, uvw=64, imh=64, imw=64, depth=64)
+        oc = ocfg(cfg)
+        params = O.init_params(oc, seed=13, dtype=torch.float64)
+        init = {k: v.clone() for k, v in params.items()}
+        m.build(5, 3)
+        m.load_params(params)
+        strategy = trainvali.Strategy()
+        opt = trainvali.Adam(learning_rate=1e-3, amsgrad=True)
+        st = {k: [torch.zeros_like(v) for _ in range(3)] for k, v in params.items()}
+        loss_rel = []
+        for step in range(1, 4):
+            bt = synth.make_batch(2, 64, 64, seed=100 + step)
+            loss, _ = trainvali.distributed_train_step(strategy, m, bt, opt, 2)
+            ps = {k: v.detach().clone().requires_grad_(True) for k, v in params.items()}
+            l64 = O.train_loss(ps, oc, tuple(t.double() if torch.is_tensor(t) else t for t in bt), 2)
+            l64.backward()
+            loss_rel.append(abs(float(loss) - float(l64)) / abs(float(l64)))
+            for k in params:
+                p, mm, v, vh = O.amsgrad_step(params[k], ps[k].grad, *st[k], step, 1e-3)
+                params[k], st[k] = p, [mm, v, vh]
+        got = m.export_params()
+        num = den = 0.0
+        out_of_band = total = 0
         for k in params:
-            p, mm, v, vh = O.amsgrad_step(params[k], ps[k].grad, *st[k], step, 1e-3)
-            params[k], st[k] = p, [mm, v, vh]
-    got = m.export_params()
-    num = den = 0.0
-    out_of_band = total = 0
-    for k in params:
-        d_got = got[k].double().cpu() - init[k]
-        d_want = params[k] - init[k]
-        num += float((d_got - d_want).pow(2).sum())
-        den += float(d_want.pow(2).sum())
-        out_of_band += int(((got[k].double().cpu() - params[k]).abs() > 5e-5).sum())
-        total += params[k].numel()
-    rel = (num / den) ** 0.5
-    _record('tc_amsgrad3', {'loss_rel_per_step': loss_rel, 'displacement_rel_fro': rel,
-                            'elements_outside_5e-5': out_of_band, 'elements': total})
-    assert max(loss_rel) <= 1e-4
-    assert rel <= 3e-2 and out_of_band <= 0.02 * total, (rel, out_of_band, total)
+            d_got = got[k].double().cpu() - init[k]
+            d_want = params[k] - init[k]
+            num += float((d_got - d_want).pow(2).sum())
+            den += float(d_want.pow(2).sum())
+            out_of_band += int(((got[k].double().cpu() - params[k]).abs() > 5e-5).sum())
+            total += params[k].numel()
+        rel = (num / den) ** 0.5
+        _record('tc_amsgrad3', {'loss_rel_per_step': loss_rel, 'displacement_rel_fro': rel,
+                                'elements_outside_5e-5': out_of_band, 'elements': total})
+        assert max(loss_rel) <= 1e-4
+        assert rel <= 3e-2 and out_of_band <= 0.02 * total, (rel, out_of_band, total)
 
 
 @pytest.mark.parametrize('over,k_obs,B', [(dict(uvh=64, uvw=64, imh=64, imw=64), 6, 2),
@@ -183,14 +183,14 @@ def test_model_backward_k_observations_and_depth_1024(over, k_obs, B):
     depth-1024 network one flipped derivative bit moves a bias gradient by a percent, which says nothing about the
     kernels."""
     import nlt_native as nat
-    nat.set_option('tc', 1)
-    m, oc, bt, params, masks, pred, per = _product_and_masks(over, B, seed=77, k_obs=k_obs)
-    p64, g64, flips = _oracle_grads(params, oc, bt, B, masks)
-    assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
-    grads = m.export_grads()
-    worst = max((rel_fro(grads[k], g64[k]), k) for k in params)
-    assert worst[0] <= 1e-4, (worst, flips)
-    assert flips['flipped'] <= 1e-4 * flips['total'] + 2, flips
+    with nat.options(tc=1):
+        m, oc, bt, params, masks, pred, per = _product_and_masks(over, B, seed=77, k_obs=k_obs)
+        p64, g64, flips = _oracle_grads(params, oc, bt, B, masks)
+        assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
+        grads = m.export_grads()
+        worst = max((rel_fro(grads[k], g64[k]), k) for k in params)
+        assert worst[0] <= 1e-4, (worst, flips)
+        assert flips['flipped'] <= 1e-4 * flips['total'] + 2, flips
 
 
 def test_full_size_sample_1024_forward_backward():
@@ -198,16 +198,16 @@ def test_full_size_sample_1024_forward_backward():
     forward within 2e-5, per-sample loss within 1e-4, weight gradients within 1e-4 given the product's own
     LeakyReLU branches (see the first test) and within 3e-3 against the plain oracle."""
     import nlt_native as nat
-    nat.set_option('tc', 1)
-    over = dict(uvh=1024, uvw=1024, imh=1024, imw=1024)
-    m, oc, bt, params, masks, pred, per = _product_and_masks(over, 1, seed=4321)
-    p64, g_masked, flips = _oracle_grads(params, oc, bt, 1, masks)
-    assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
-    grads = m.export_grads()
-    worst = max((rel_fro(grads[k], g_masked[k]), k) for k in params)
-    _record('full_size_1024', {'worst_rel_fro_with_product_masks': worst[0], 'layer': worst[1],
-                               'flipped_bits': flips['flipped'], 'activation_elements': flips['total']})
-    assert worst[0] <= 1e-4, worst
+    with nat.options(tc=1):
+        over = dict(uvh=1024, uvw=1024, imh=1024, imw=1024)
+        m, oc, bt, params, masks, pred, per = _product_and_masks(over, 1, seed=4321)
+        p64, g_masked, flips = _oracle_grads(params, oc, bt, 1, masks)
+        assert float((pred.double().cpu() - p64).abs().max()) <= 2e-5
+        grads = m.export_grads()
+        worst = max((rel_fro(grads[k], g_masked[k]), k) for k in params)
+        _record('full_size_1024', {'worst_rel_fro_with_product_masks': worst[0], 'layer': worst[1],
+                                   'flipped_bits': flips['flipped'], 'activation_elements': flips['total']})
+        assert worst[0] <= 1e-4, worst
 
 
 def test_graph_replay_equals_eager_and_survives_scratch_regrowth():

@@ -228,38 +228,37 @@ def _product(monkeypatch, over, B, seed, tc):
     import engine
     import nlt_native as nat
     from util import synth
-    nat.set_option('tc', tc)
-    m, cfg = make_model(**over)
-    oc = ocfg(cfg)
-    bt = synth.make_batch(B, oc['uvh'], oc['imh'], seed=seed)
-    params = P.init_params(oc, seed=7, dtype=torch.float64)
-    m.build(5, 3)
-    m.load_params(params)
-    masks, args = {}, {}
-    conv_fwd, norm_fwd, pool_fwd = engine.ConvLayer.forward, engine.NormLayer.forward, engine.PoolLayer.forward
+    with nat.options(tc=tc):
+        m, cfg = make_model(**over)
+        oc = ocfg(cfg)
+        bt = synth.make_batch(B, oc['uvh'], oc['imh'], seed=seed)
+        params = P.init_params(oc, seed=7, dtype=torch.float64)
+        m.build(5, 3)
+        m.load_params(params)
+        masks, args = {}, {}
+        conv_fwd, norm_fwd, pool_fwd = engine.ConvLayer.forward, engine.NormLayer.forward, engine.PoolLayer.forward
 
-    def tap(layer, out):
-        if layer.act is not None:
-            masks[layer.name.split(' ')[0].replace('.norm', '')] = (out.t > 0).cpu()
-        return out
-    monkeypatch.setattr(engine.ConvLayer, 'forward', lambda self, segs, tape=None: tap(self, conv_fwd(self, segs, tape)))
-    monkeypatch.setattr(engine.NormLayer, 'forward', lambda self, x, tape=None: tap(self, norm_fwd(self, x, tape)))
+        def tap(layer, out):
+            if layer.act is not None:
+                masks[layer.name.split(' ')[0].replace('.norm', '')] = (out.t > 0).cpu()
+            return out
+        monkeypatch.setattr(engine.ConvLayer, 'forward', lambda self, segs, tape=None: tap(self, conv_fwd(self, segs, tape)))
+        monkeypatch.setattr(engine.NormLayer, 'forward', lambda self, x, tape=None: tap(self, norm_fwd(self, x, tape)))
 
-    def pool_forward(self, x, tape=None):
-        if self.kind == 'max':
-            args[self.name.split(' ')[0]] = P.first_argmax(x.t).cpu()
-        return pool_fwd(self, x, tape)
-    monkeypatch.setattr(engine.PoolLayer, 'forward', pool_forward)
-    try:
-        pred, gt, kw, _ = m(bt, mode='train')
-        kw['keep_batch'] = True
-        m.set_loss_grad_scale(1.0 / B)
-        m.compute_loss(pred, gt, **kw)
-        m.backward()
-        torch.cuda.synchronize()
-    finally:
-        monkeypatch.undo()
-        nat.set_option('tc', 1)
+        def pool_forward(self, x, tape=None):
+            if self.kind == 'max':
+                args[self.name.split(' ')[0]] = P.first_argmax(x.t).cpu()
+            return pool_fwd(self, x, tape)
+        monkeypatch.setattr(engine.PoolLayer, 'forward', pool_forward)
+        try:
+            pred, gt, kw, _ = m(bt, mode='train')
+            kw['keep_batch'] = True
+            m.set_loss_grad_scale(1.0 / B)
+            m.compute_loss(pred, gt, **kw)
+            m.backward()
+            torch.cuda.synchronize()
+        finally:
+            monkeypatch.undo()
     return m, oc, bt, params, masks, args, pred
 
 

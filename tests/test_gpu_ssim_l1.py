@@ -156,24 +156,24 @@ def test_model_train_step(loss, monkeypatch):
     import nlt_native as nat
     from tests.test_gpu_model import rel_fro
     from tests.test_gpu_parity import _oracle_grads, _product_and_masks
-    nat.set_option('tc', 1)
-    B = 2
-    m, oc, bt, params, masks, pred, per = _product_and_masks(dict(uvh=64, uvw=64, imh=64, imw=64, loss=loss), B,
-                                                             seed=77)
-    objective = _oracle_objective(loss)
-    monkeypatch.setattr(O, 'l2_loss', objective)          # _oracle_grads differentiates sum_b O.l2_loss(...) / B
-    p64, g_masked, flips = _oracle_grads(params, oc, bt, B, masks)
-    bt64 = tuple(t.double() if torch.is_tensor(t) else t for t in bt)
-    with torch.no_grad():
-        pr, gt, _, _ = O.model_call(params, oc, bt64, 'train')
-        want = objective(gt, pr)
-    loss_err = float(((per.double().cpu() - want) / want).abs().max())
-    grads = m.export_grads()
-    worst = max(rel_fro(grads[k], g_masked[k]) for k in params)
-    RECORD['model %s' % loss] = {'loss_rel_err': loss_err, 'worst_wgrad_rel_fro_masked': worst,
-                                 'flipped_bits': flips['flipped']}
-    _record()
-    assert loss_err <= 1e-4 and worst <= 1e-4, RECORD['model %s' % loss]
+    with nat.options(tc=1):
+        B = 2
+        m, oc, bt, params, masks, pred, per = _product_and_masks(dict(uvh=64, uvw=64, imh=64, imw=64, loss=loss), B,
+                                                                 seed=77)
+        objective = _oracle_objective(loss)
+        monkeypatch.setattr(O, 'l2_loss', objective)          # _oracle_grads differentiates sum_b O.l2_loss(...) / B
+        p64, g_masked, flips = _oracle_grads(params, oc, bt, B, masks)
+        bt64 = tuple(t.double() if torch.is_tensor(t) else t for t in bt)
+        with torch.no_grad():
+            pr, gt, _, _ = O.model_call(params, oc, bt64, 'train')
+            want = objective(gt, pr)
+        loss_err = float(((per.double().cpu() - want) / want).abs().max())
+        grads = m.export_grads()
+        worst = max(rel_fro(grads[k], g_masked[k]) for k in params)
+        RECORD['model %s' % loss] = {'loss_rel_err': loss_err, 'worst_wgrad_rel_fro_masked': worst,
+                                     'flipped_bits': flips['flipped']}
+        _record()
+        assert loss_err <= 1e-4 and worst <= 1e-4, RECORD['model %s' % loss]
 
 
 # ---------------------------------------------------------------------------
