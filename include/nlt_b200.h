@@ -229,6 +229,31 @@ int nlt_barron_loss(const float* pred, const float* gt, const float* alpha, int3
                     int32_t levels, float scale, float log_z, float loss_scale, float* loss, float* d_pred,
                     void* workspace, void* stream);
 
+/* losses.LPIPS (nlt/losses.py:143-169) per sample, fused with its input gradient: the frozen LPIPS AlexNet graph
+ * third_party/lpips/net-lin_alex_v0.1.pb of the reference, with pred as its input 0 and gt as its input 1:
+ *   x = (2 v - 1) * scale_c + shift_c ; conv1 11x11/s4 pad 2 -> ReLU -> maxpool 3x3/s2 ; conv2 5x5 pad 2 -> ReLU ->
+ *   maxpool ; conv3, conv4, conv5 3x3 pad 1 -> ReLU ; per ReLU output f_l:  u = f / (|f|_c + 1e-10),
+ *   loss[b] = sum_l mean_{h,w} sum_c lin_l[c] (u_pred - u_gt)^2 ;  d_pred = d(sum_b loss[b] * loss_scale) / d(pred)
+ * Where every channel of a pred feature vector is 0 the normalisation's gradient term is taken as 0 (the reference's
+ * TF gradient is NaN there).  pred, gt: [B,H,W,3] with H, W >= 31 and B <= 65535; d_pred may be NULL (the loss is
+ * bit-identical either way).  Deterministic: per-block partials summed per sample in a fixed order, in double.
+ * Weights are device pointers in the graph's own layouts (kernels OIHW [Cout][Cin][k][k]).  workspace >=
+ * nlt_lpips_loss_workspace_bytes() (< 0 for a refused shape), contents on entry irrelevant.  No weight gradients.
+ * After a call the workspace, from its first 256-byte boundary on, holds the network's activations of all 2B images
+ * (pred first), each starting at the next 256-byte boundary: x [2B,H,W,3], relu1, pool1, relu2, pool2, relu3, relu4,
+ * relu5 (NHWC); tests read the ReLU masks of the pred half from there. */
+typedef struct nlt_lpips_weights {
+  const float* scale;   /* [3] */
+  const float* shift;   /* [3] */
+  const float* w[5];    /* [64,3,11,11] [192,64,5,5] [384,192,3,3] [256,384,3,3] [256,256,3,3] */
+  const float* b[5];    /* [Cout] */
+  const float* lin[5];  /* [Cout], the distance head's channel weights */
+} nlt_lpips_weights;
+int64_t nlt_lpips_loss_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int nlt_lpips_loss(const float* pred, const float* gt, const nlt_lpips_weights* weights, int32_t B, int32_t H,
+                   int32_t W, float loss_scale, float* loss, float* d_pred, void* workspace, int64_t workspace_bytes,
+                   void* stream);
+
 /* tf.keras.optimizers.Adam(lr, amsgrad=True) dense update over a flat bucket
  * (nlt/trainvali.py:122-127, 280); step is 1-based; grad_scale multiplies g. */
 int nlt_amsgrad_step(float* p, const float* g, float* m, float* v, float* vhat,

@@ -6,7 +6,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -I../../include"
 OBJS=""
 PIDS=""
-for f in nlt_gconv nlt_ops nlt_small nlt_tc nlt_barron nlt_ssim nlt_pwx nlt_norm nlt_tiny nlt_wop nlt_pool ${NLT_EXTRA_SRCS}; do
+for f in nlt_gconv nlt_ops nlt_small nlt_tc nlt_barron nlt_ssim nlt_pwx nlt_norm nlt_tiny nlt_wop nlt_pool nlt_lpips ${NLT_EXTRA_SRCS}; do
   if [ ! -f $f.o ] || [ $f.cu -nt $f.o ] || [ nlt_common.cuh -nt $f.o ] || [ nlt_barron_core.h -nt $f.o ] || [ ../../include/nlt_b200.h -nt $f.o ] || [ build.sh -nt $f.o ]; then
     echo "nvcc $f.cu"
     if [ -n "${NLT_PTXAS_V}" ]; then

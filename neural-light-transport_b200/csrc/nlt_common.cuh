@@ -231,11 +231,19 @@ int launch_pws_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size
 
 // wgmma tensor-core path (nlt_tc.cu)
 extern unsigned long long g_tc_launches;
-bool tc_applicable(const GConvK& k);
-size_t tc_workspace_bytes(const GConvK& k);
+// partial_tiles: also lattices that are not a multiple of the tile shape (edge tiles partly masked)
+bool tc_applicable(const GConvK& k, bool partial_tiles = false);
+size_t tc_workspace_bytes(const GConvK& k, bool partial_tiles = false);
 int launch_tc(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act, float* out,
-              void* workspace, size_t workspace_bytes, cudaStream_t st, bool prepacked = false);
-int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream_t st);
+              void* workspace, size_t workspace_bytes, cudaStream_t st, bool prepacked = false, bool partial_tiles = false);
+int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream_t st, bool partial_tiles = false);
+
+// A forward or input-gradient op of the public descriptor form, routed as nlt_gconv_fwd_ws routes it, for the library's
+// own composite ops (nlt_lpips.cu).  partial_tiles: the wgmma kernel also takes lattices that are not a multiple of
+// its tile shape.  gconv_tc_workspace_bytes: the scratch that op needs on the wgmma kernel (0 when it cannot run there).
+int gconv_run(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y, int mask_act,
+              float* out, void* workspace, int64_t workspace_bytes, bool partial_tiles, cudaStream_t st);
+int64_t gconv_tc_workspace_bytes(const nlt_gconv_desc* d, bool partial_tiles);
 
 bool tc_wgrad_applicable(const GConvK& k);
 size_t tc_wgrad_ws_floats(const GConvK& k);

@@ -755,11 +755,12 @@ static Route pwd2s_route() { return opt(Opt::TC) && opt(Opt::PWMMA) ? Route::PWD
 // takes its phase_route.  The wgmma kernel needs its workspace within `ws_bytes` (< 0: no workspace, so the op stays
 // on the fp32 kernels).
 static Route fwd_route(const GConvK* ph, int np, const float* bias, int act, float beta, const float* mask_y,
-                       const float* out, int64_t ws_bytes) {
+                       const float* out, int64_t ws_bytes, bool partial_tiles = false) {
   if (np != 1 || ph[0].M == 0) return Route::NONE;
   const GConvK& k = ph[0];
   auto tc = [&] {
-    return opt(Opt::TC) && tc_applicable(k) && ws_bytes >= 0 && (int64_t)tc_workspace_bytes(k) <= ws_bytes;
+    return opt(Opt::TC) && tc_applicable(k, partial_tiles) && ws_bytes >= 0 &&
+           (int64_t)tc_workspace_bytes(k, partial_tiles) <= ws_bytes;
   };
   if (opt(Opt::TC) == 2 && tc()) return Route::TC;
   // staged-patch forward; its stride-1 form only with pf_s1
@@ -803,9 +804,10 @@ static Route fused_route(const GConvK& k, const PwExtra& ex, const float* bias, 
 
 static int launch_route(Route r, const GConvK& k, const float* bias, int act, float beta, const float* mask_y,
                         int mask_act, float* out, const PwExtra* ex, void* ws, int64_t ws_bytes, bool prepacked,
-                        cudaStream_t st) {
+                        cudaStream_t st, bool partial_tiles = false) {
   switch (r) {
-    case Route::TC: return launch_tc(k, bias, act, beta, mask_y, mask_act, out, ws, (size_t)ws_bytes, st, prepacked);
+    case Route::TC:
+      return launch_tc(k, bias, act, beta, mask_y, mask_act, out, ws, (size_t)ws_bytes, st, prepacked, partial_tiles);
     case Route::PF: return launch_pf_fwd(k, bias, act, beta, mask_y, mask_act, out, st);
     case Route::TINY: return launch_tiny_stencil(k, bias, act, beta, mask_y, mask_act, out, st);
     case Route::PWX: return launch_pwx_fwd(k, bias, act, out, st);
@@ -939,7 +941,8 @@ int nlt_gconv_pack_weights(const nlt_gconv_desc* d, void* packed, int64_t packed
 }
 
 static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y,
-                          int mask_act, float* out, void* workspace, int64_t workspace_bytes, void* stream, bool prepacked) {
+                          int mask_act, float* out, void* workspace, int64_t workspace_bytes, void* stream, bool prepacked,
+                          bool partial_tiles = false) {
   GConvK ph[16];
   int np = 0;
   int rc = build_phases(d, ph, &np, /*allow_d2s=*/true);
@@ -951,13 +954,13 @@ static int gconv_fwd_impl(const nlt_gconv_desc* d, const float* bias, int act, f
   // packed weights are only for an op that nlt_gconv_fwd_pack_bytes puts on the wgmma kernel: route it as that query
   // does (no bias)
   const Route r = fwd_route(ph, np, prepacked ? nullptr : bias, prepacked ? 0 : act, beta, mask_y, out,
-                            workspace != nullptr ? workspace_bytes : -1);
+                            workspace != nullptr ? workspace_bytes : -1, partial_tiles);
   if (prepacked)
     NLT_CHECK_ARG(r != Route::NONE && r != Route::PWD2S,
                   "nlt_gconv_fwd_packed: this op does not run on the tensor-core kernel (nlt_gconv_fwd_pack_bytes == 0)");
   if (r != Route::NONE)
     return launch_route(r, ph[0], bias, act, beta, mask_y, mask_act, out, nullptr, workspace, workspace_bytes, prepacked,
-                        st);
+                        st, partial_tiles);
   for (int i = 0; i < np; ++i) {
     const GConvK& k = ph[i];
     if (k.M == 0) continue;
@@ -1097,3 +1100,19 @@ int nlt_gconv_wgrad(const nlt_gconv_desc* d, const float* G, float* dW, float* d
 }
 
 }  // extern "C"
+
+namespace nlt {
+
+int gconv_run(const nlt_gconv_desc* d, const float* bias, int act, float beta, const float* mask_y, int mask_act,
+              float* out, void* workspace, int64_t workspace_bytes, bool partial_tiles, cudaStream_t st) {
+  return gconv_fwd_impl(d, bias, act, beta, mask_y, mask_act, out, workspace, workspace_bytes, st, false, partial_tiles);
+}
+
+int64_t gconv_tc_workspace_bytes(const nlt_gconv_desc* d, bool partial_tiles) {
+  GConvK ph[16];
+  int np = 0;
+  if (build_phases(d, ph, &np, /*allow_d2s=*/true) != NLT_OK) return -1;
+  return np == 1 && tc_applicable(ph[0], partial_tiles) ? (int64_t)tc_workspace_bytes(ph[0], partial_tiles) : 0;
+}
+
+}  // namespace nlt

@@ -525,7 +525,7 @@ static int pick_bn(int cout) {
 }
 
 // Which single-phase GConvK shapes the tensor path takes (everything else stays on the SIMT kernels).
-static TcPlan tc_plan(const GConvK& k) {
+static TcPlan tc_plan(const GConvK& k, bool partial_tiles) {
   TcPlan pl;
   memset(&pl, 0, sizeof(pl));
   pl.ok = false;
@@ -559,13 +559,13 @@ static TcPlan tc_plan(const GConvK& k) {
   // tile shape
   // tile shape: TW = 128 lattice columns, or the smallest power of two >= Wl; partial tiles at the right / bottom
   // edge load zeros (TMA out-of-bounds fill) or rows that only feed masked outputs, and store nothing outside.
-  // Only option tc = 2 takes lattices that are not a multiple of the tile shape: at the 1x1 .. 4x4 bottleneck levels
-  // most rows of a tile would be masked, and the fp32 kernels serve those layers
+  // Only option tc = 2 and callers that ask for partial tiles take lattices that are not a multiple of the tile shape:
+  // at the 1x1 .. 4x4 bottleneck levels most rows of a tile would be masked, and the fp32 kernels serve those layers
   if (p.Hl < 1 || p.Wl < 1) return pl;
   p.TW = TC_BM;
   while (p.TW / 2 >= p.Wl) p.TW /= 2;
   p.TH = TC_BM / p.TW;
-  if (!force && (p.Wl % p.TW != 0 || p.Hl % p.TH != 0)) return pl;
+  if (!force && !partial_tiles && (p.Wl % p.TW != 0 || p.Hl % p.TH != 0)) return pl;
   p.tiles_x = (p.Wl + p.TW - 1) / p.TW; p.tiles_y = (p.Hl + p.TH - 1) / p.TH;
   // coordinate map
   const bool stride1 = (k.ay.it == 1 && k.ax.it == 1);
@@ -1126,10 +1126,10 @@ int launch_tc_wgrad(const GConvK& k, const float* G, float* ws, WgradK* w, size_
   }
 }
 
-bool tc_applicable(const GConvK& k) { return tc_plan(k).ok; }
+bool tc_applicable(const GConvK& k, bool partial_tiles) { return tc_plan(k, partial_tiles).ok; }
 
-size_t tc_workspace_bytes(const GConvK& k) {
-  TcPlan pl = tc_plan(k);
+size_t tc_workspace_bytes(const GConvK& k, bool partial_tiles) {
+  TcPlan pl = tc_plan(k, partial_tiles);
   return pl.ok ? 2 * pl.pack_floats * sizeof(float) + 256 : 0;
 }
 
@@ -1156,8 +1156,8 @@ static int tc_launch_bn(const TcMaps& maps, const TcPlan& pl, cudaStream_t st) {
 }
 
 // hi / lo planes of the weights in K-block layout (what the B tensor maps of the conv kernel read)
-int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-  TcPlan pl = tc_plan(k);
+int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream_t st, bool partial_tiles) {
+  TcPlan pl = tc_plan(k, partial_tiles);
   if (!pl.ok) return set_err(NLT_ERR_INVALID, "tensor-core path not applicable");
   const size_t need = 2 * pl.pack_floats * sizeof(float) + 256;
   NLT_CHECK_ARG(workspace != nullptr && workspace_bytes >= need, "tc workspace too small: need %zu", need);
@@ -1172,15 +1172,15 @@ int tc_pack(const GConvK& k, void* workspace, size_t workspace_bytes, cudaStream
 }
 
 int launch_tc(const GConvK& k, const float* bias, int act, float beta, const float* mask_y, int mask_act, float* out,
-              void* workspace, size_t workspace_bytes, cudaStream_t st, bool prepacked) {
-  TcPlan pl = tc_plan(k);
+              void* workspace, size_t workspace_bytes, cudaStream_t st, bool prepacked, bool partial_tiles) {
+  TcPlan pl = tc_plan(k, partial_tiles);
   if (!pl.ok) return set_err(NLT_ERR_INVALID, "tensor-core path not applicable");
   const size_t need = 2 * pl.pack_floats * sizeof(float) + 256;
   NLT_CHECK_ARG(workspace != nullptr && workspace_bytes >= need, "tc workspace too small: need %zu", need);
   float* bhi = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(workspace) + 255) & ~(uintptr_t)255);
   float* blo = bhi + pl.pack_floats;
   if (!prepacked) {
-    const int rc0 = tc_pack(k, workspace, workspace_bytes, st);
+    const int rc0 = tc_pack(k, workspace, workspace_bytes, st, partial_tiles);
     if (rc0 != NLT_OK) return rc0;
   }
   TcMaps maps;

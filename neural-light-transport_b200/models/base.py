@@ -9,7 +9,6 @@ _MODES = ('train', 'vali', 'test')
 
 # loss name -> constructor (nlt/models/base.py:41-61; 'elpips' needs the TF-only E-LPIPS package and is not offered)
 _LOSS_TABLE = {
-    'lpips': lambda: losses.LPIPS(per_ch=False),
     'l1': lambda: losses.L1(),
     'l2': lambda: losses.L2(),
     'ssim': lambda: losses.SSIM(1 - 0),
@@ -37,6 +36,9 @@ class Model:
             name, weight = self._parse_loss_and_weight(item)
             if name == 'barron':     # needs the image size (nlt/models/nlt.py:78-79); experimental, see losses.Barron
                 loss = losses.Barron(self.config.getint('DEFAULT', 'imw'), self.config.getint('DEFAULT', 'imh'))
+            elif name == 'lpips':    # needs the reference's frozen graph, which is not shipped: see losses.LPIPS
+                loss = losses.LPIPS(per_ch=False,
+                                    weights_path=self.config.get('DEFAULT', losses.LPIPS.KEY, fallback=None))
             elif name in _LOSS_TABLE:
                 loss = _LOSS_TABLE[name]()
             else:

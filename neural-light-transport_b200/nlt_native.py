@@ -40,6 +40,12 @@ class PwTerm(C.Structure):
                 ('w_k_stride', C.c_int64), ('w_n_stride', C.c_int64)]
 
 
+class LpipsWeights(C.Structure):
+    """nlt_lpips_weights (include/nlt_b200.h): device pointers to the LPIPS AlexNet constants."""
+    _fields_ = [('scale', C.c_void_p), ('shift', C.c_void_p), ('w', C.c_void_p * 5), ('b', C.c_void_p * 5),
+                ('lin', C.c_void_p * 5)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -89,6 +95,9 @@ _SIGS = {
                               C.c_void_p, C.c_void_p]),
     'nlt_ssim_loss_workspace_bytes': (C.c_int64, [C.c_int32] * 3),
     'nlt_ssim_loss': (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_float] * 2 + [C.c_void_p] * 4),
+    'nlt_lpips_loss_workspace_bytes': (C.c_int64, [C.c_int32] * 3),
+    'nlt_lpips_loss': (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(LpipsWeights)] + [C.c_int32] * 3
+                       + [C.c_float] + [C.c_void_p] * 3 + [C.c_int64, C.c_void_p]),
     'nlt_amsgrad_step': (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_int32] + [C.c_float] * 5 + [C.c_void_p]),
     'nlt_amsgrad_step_dev': (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_void_p] + [C.c_float] * 5 + [C.c_void_p]),
     'nlt_pixelnorm_fwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_int, C.c_void_p, C.c_void_p]),
